@@ -20,9 +20,11 @@ using namespace sb;
 
 struct sb_frame {
   sb_ctx* ctx;
-  FrameDev d;
-  float4* base;
+  uint64_t id;  // unique within the context, never reused (keys the render memo)
+  FrameDev d;   // views into base
+  DevPtr<float4> base;
 };
+using FramePtr = Owned<sb_frame, std::default_delete<sb_frame>>;
 
 struct DevTile {  // SubmapCache, SurfelMap.h:179-181 -- kept in HBM (tile pool) instead of host RAM
   uint32_t slot = 0;
@@ -43,16 +45,16 @@ struct sb_ctx {
   // ---- preprocessing scratch
   PrepKeys prep;            // two alternating z-buffer key images of the scan projection (+ TMA maps)
   bool prepped_for_update = false;  // radius map / index keys / integrated flags of c->cur are ready (pipeline mode)
-  float4* d_pts = nullptr;
-  float* d_labels = nullptr;
-  float* d_probs = nullptr;
+  DevPtr<float4> d_pts;
+  DevPtr<float> d_labels;
+  DevPtr<float> d_probs;
   size_t pts_cap = 0;
   // optional input prefetch (sb_prefetch_scan): a ring of staging buffers filled on a copy stream while the previous
   // scan is being processed; created on first use, the default path never touches it
   struct PrefetchSlot {
-    float4* pts = nullptr;
-    float* labels = nullptr;
-    float* probs = nullptr;
+    DevPtr<float4> pts;
+    DevPtr<float> labels;
+    DevPtr<float> probs;
     const float* host_pts = nullptr;
     uint32_t n = 0;
     bool has_labels = false, has_probs = false, valid = false, in_use = false;
@@ -64,80 +66,95 @@ struct sb_ctx {
   cudaStream_t copy_stream = nullptr;
 
   // ---- ICP
-  GnState* gn = nullptr;
-  GnState* gn2 = nullptr;  // state of the frame-to-frame fallback minimisation
-  long long* acc32 = nullptr;
-  long long* acc_slots = nullptr;  // per-block partial sums of the Jacobian kernels (1024 x 32 int64)
-  unsigned int* ticket = nullptr;
-  void* h_pinned = nullptr;  // pinned staging for small read-backs (64 KiB)
+  DevPtr<GnState> gn;
+  DevPtr<GnState> gn2;  // state of the frame-to-frame fallback minimisation
+  DevPtr<long long> acc_slots;  // per-block partial sums of the Jacobian kernels (1024 x 32 int64)
+  DevPtr<unsigned int> ticket;
+  // pinned staging of the small read-backs and uploads; one member per transfer, so none overlaps another
+  struct Staging {
+    ResultBlock result;                      // mirror of the per-scan result block (also stages the initial pose block)
+    GnHead gn;                               // head of a Gauss-Newton state
+    long long sums[32];                      // raw sums of one Jacobian pass
+    double history[(kMaxGnIter + 1) * 16];   // poses of a host-driven Gauss-Newton run
+  };
+  PinnedPtr<Staging> host;
   int icp_blocks = 296;
-  int icp_coop_blocks = 0;  // > 0: the persistent cooperative Gauss-Newton kernel is available
+  int icp_coop_blocks = 0;  // grid of the persistent cooperative Gauss-Newton kernel
   unsigned int epoch_base = 1;  // epoch words of the persistent GN kernel: each launch owns a fresh range of values
-  unsigned long long* gn_pub = nullptr;  // 32 (half pose value, epoch tag) words published by every Gauss-Newton step
-  int gn_use_cache = 1;                  // SUMA_B200_GN_CACHE = 0: reload the data texels every iteration (measurement switch)
+  DevPtr<unsigned long long> gn_pub;  // 32 (half pose value, epoch tag) words published by every Gauss-Newton step
   // loop closure (SurfelMapping::checkLoopClosure; include/suma_b200_loop.hpp): off unless sb_set_loop_closure enables it
   bool close_loops = false;
   suma_b200::loop::State loop;
   double lastPose_old[16];
 
   // ---- map
-  SurfelPlanes A{}, T{}, G{}, X{};  // current surfels, updated (same index), generated (per pixel), extraction buffer
-  uint8_t* keep = nullptr;
-  uint32_t* block_counts = nullptr;
-  uint32_t* block_offsets = nullptr;
-  unsigned long long* lb_desc = nullptr;  // look-back descriptors of the single-pass compactions
-  uint32_t* lb_ticket = nullptr;
+  // current surfels, updated (same index), generated (per pixel), extraction buffer: views into the *_mem allocations
+  SurfelPlanes A{}, T{}, G{}, X{};
+  DevPtr<float4> A_mem, T_mem, G_mem, X_mem;
+  DevPtr<uint8_t> keep;
+  DevPtr<uint32_t> block_counts;
+  DevPtr<uint32_t> block_offsets;
+  DevPtr<unsigned long long> lb_desc;  // look-back descriptors of the single-pass compactions
+  DevPtr<uint32_t> lb_ticket;
   uint32_t lb_gen = 0;
-  uint32_t* d_counts = nullptr;  // [0] n surfels, [1] n after update (base for new), [2] kept updated, [3] kept new, [4] extracted
-  float* poses = nullptr;        // device pose table, kMaxPoses x 16
-  float* poses_inv = nullptr;
+  DevPtr<ResultBlock> res;  // pose block, statistics sums and surfel counts of the scan
+  DevPtr<float> poses;      // device pose table, kMaxPoses x 16
+  DevPtr<float> poses_inv;
   std::vector<float> h_poses, h_poses_inv;
-  float* Mtab_old = nullptr;
-  float* Mtab_new = nullptr;
-  unsigned long long* key_old = nullptr;  // three model-size key images, contiguous
+  DevPtr<float> Mtab_old;
+  DevPtr<float> Mtab_new;
+  DevPtr<unsigned long long> key_old;  // three model-size key images, contiguous
   unsigned long long* key_new = nullptr;
   unsigned long long* key_comp = nullptr;
-  unsigned long long* key_index = nullptr;
-  float4* radius_map = nullptr;
-  uint8_t* integrated = nullptr;
-  uint32_t* group_counts = nullptr;  // kGroupCounts totals of the update pass (64 blocks each)
-  sb_frame* f_old = nullptr;
-  sb_frame* f_new = nullptr;
-  sb_frame* f_comp = nullptr;
+  DevPtr<unsigned long long> key_index;
+  DevPtr<float4> radius_map;
+  DevPtr<uint8_t> integrated;
+  DevPtr<uint32_t> group_counts;  // kGroupCounts totals of the update pass (64 blocks each)
+  FramePtr f_old, f_new, f_comp;
+  uint64_t frames_created = 0;
   uint32_t n_host = 0;   // surfel count (exact; refreshed after every update)
   uint32_t n_upper = 0;  // upper bound used for grid sizing while the exact count is still in flight
-  char* result_block = nullptr;  // pd | acc32 | d_counts in one allocation (one device-to-host copy per scan)
-  PoseDev* pd = nullptr; // device-resident pose bookkeeping of the pipeline
   uint32_t n_updated = 0, n_new = 0;
   uint32_t map_timestamp = 0;
   int32_t origin_i = 0, origin_j = 0;
   std::vector<std::pair<int32_t, int32_t>> extraction;
   std::map<std::pair<int32_t, int32_t>, DevTile> tiles;
   SurfelPlanes pool{};            // tile cache lanes
-  uint32_t* d_pool_top = nullptr;
-  uint2* d_tile_rec = nullptr;    // {base, count} per extraction
+  DevPtr<float4> pool_mem;
+  DevPtr<uint32_t> d_pool_top;
+  DevPtr<uint2> d_tile_rec;       // {base, count} per extraction
   uint32_t n_slots = 0;
   bool tiles_pending = false;     // some records have not been read back yet
 
-  // full-render memo: SurfelMapping re-renders the unchanged map at the unchanged pose at the start of the next scan
-  // (SurfelMapping.cpp:351 after :803); identical arguments on an unmodified map reproduce identical images
-  struct RenderKey {
-    float pose_old[16], pose_new[16];
-    float conf_thr;
-    uint32_t map_timestamp;
-    uint64_t map_version;
-    int compose;
-    const sb_frame* out;
-  } rkey{};
-  bool rkey_valid = false;
+  // Full-render memo: SurfelMapping re-renders the unchanged map at the unchanged pose at the start of the next scan
+  // (SurfelMapping.cpp:351 after :803); identical arguments on an unmodified map reproduce identical images. The memo
+  // holds while nothing but that render has written the frames it covers (old, new, composed and `out`: see
+  // frame_written) and nothing the render reads has changed (map_version, sb_set_params, sb_set_current_pose).
+  struct RenderMemo {
+    struct Key {
+      float pose_old[16], pose_new[16];
+      float conf_thr;
+      uint32_t map_timestamp;
+      uint64_t map_version;
+      uint64_t out;  // sb_frame::id
+      int compose;
+      int pad;       // no padding bytes: keys are compared with memcmp
+    };
+    static_assert(sizeof(Key) == 160, "RenderMemo::Key has padding");
+    Key key{};
+    bool valid = false;
+    bool matches(const Key& k) const { return valid && memcmp(&key, &k, sizeof(k)) == 0; }
+    void store(const Key& k) {
+      key = k;
+      valid = true;
+    }
+    void clear() { valid = false; }
+  } memo;
   uint64_t map_version = 0;
   uint64_t renders_skipped = 0;
 
   // ---- SurfelMapping state
-  sb_frame* cur = nullptr;
-  sb_frame* last = nullptr;
-  sb_frame* cur_model = nullptr;
-  sb_frame* last_model = nullptr;
+  FramePtr cur, last, cur_model, last_model;
   uint32_t timestamp = 0;
   double currentPose[16], lastPose[16], currentPose_old[16], currentPose_new[16], lastIncrement[16];
   float confidence_threshold = 0.f, log_unstable_slam = 0.f;
@@ -146,8 +163,8 @@ struct sb_ctx {
   bool cur_has_semantics = false, last_has_semantics = false;
 
   // ---- multi-GPU
-  long long* mailbox = nullptr;
-  unsigned int* comm_epoch = nullptr;
+  DevPtr<long long> mailbox;
+  DevPtr<unsigned int> comm_epoch;
   CommDev comm{};
   bool comm_on = false;
   sb_allreduce_fn comm_cb = nullptr;  // host-side exchange (baseline); exclusive with the fused peer-memory mode
@@ -222,60 +239,35 @@ void derive(sb_ctx* c) {
   c->log_unstable_slam = logf(pu / (1.0f - pu));     // SurfelMapping.cpp:108-109
 }
 
-int alloc_planes(sb_ctx* c, SurfelPlanes* s, size_t n) {
-  float4* base = nullptr;
-  SB_CUDA(c, cudaMalloc(&base, n * 4 * sizeof(float4)));
-  s->p0 = base; s->p1 = base + n; s->p2 = base + 2 * n; s->p3 = base + 3 * n;
+int alloc_planes(sb_ctx* c, DevPtr<float4>& mem, SurfelPlanes* s, size_t n) {
+  SB_CUDA(c, dev_alloc(mem, n * 4 * sizeof(float4)));
+  s->p0 = mem; s->p1 = mem + n; s->p2 = mem + 2 * n; s->p3 = mem + 3 * n;
   return SB_OK;
 }
-void free_planes(SurfelPlanes* s) {
-  if (s->p0) cudaFree(s->p0);
-  s->p0 = s->p1 = s->p2 = s->p3 = nullptr;
-}
 
-int frame_create(sb_ctx* c, int w, int h, sb_frame** out) {
-  if (!c || w <= 0 || h <= 0 || !out) return fail(c, SB_ERR_INVALID, "frame_create: bad arguments");
-  sb_frame* f = new sb_frame();
+int frame_create(sb_ctx* c, int w, int h, FramePtr& out) {
+  if (!c || w <= 0 || h <= 0) return fail(c, SB_ERR_INVALID, "frame_create: bad arguments");
+  FramePtr f(new sb_frame());
   f->ctx = c;
+  f->id = ++c->frames_created;
   size_t P = (size_t)w * h;
-  cudaError_t e = cudaMalloc(&f->base, P * 3 * sizeof(float4));
-  if (e != cudaSuccess) {
-    delete f;
-    return fail(c, SB_ERR_NOMEM, std::string("frame alloc: ") + cudaGetErrorString(e));
-  }
+  cudaError_t e = dev_alloc(f->base, P * 3 * sizeof(float4));
+  if (e != cudaSuccess) return fail(c, SB_ERR_NOMEM, std::string("frame alloc: ") + cudaGetErrorString(e));
   cudaMemsetAsync(f->base, 0, P * 3 * sizeof(float4), c->stream);
   f->d.W = w; f->d.H = h;
   f->d.vertex = f->base; f->d.normal = f->base + P; f->d.semantic = f->base + 2 * P;
-  *out = f;
+  out = std::move(f);
   return SB_OK;
 }
 
-int release_buffers(sb_ctx* c) {
-  cudaFree(c->prep.img[0]); cudaFree(c->prep.img[1]);
-  cudaFree(c->d_pts); cudaFree(c->d_labels); cudaFree(c->d_probs);
-  cudaFree(c->gn); cudaFree(c->gn2); cudaFree(c->acc_slots); cudaFree(c->ticket); cudaFree(c->gn_pub);
-  if (c->h_pinned) cudaFreeHost(c->h_pinned);
-  free_planes(&c->A); free_planes(&c->T); free_planes(&c->G); free_planes(&c->X); free_planes(&c->pool);
-  cudaFree(c->d_pool_top); cudaFree(c->d_tile_rec);
-  cudaFree(c->keep); cudaFree(c->block_counts); cudaFree(c->block_offsets);
-  cudaFree(c->lb_desc); cudaFree(c->lb_ticket);
-  cudaFree(c->poses); cudaFree(c->poses_inv); cudaFree(c->Mtab_old); cudaFree(c->Mtab_new);
-  cudaFree(c->key_old); cudaFree(c->key_index); cudaFree(c->radius_map); cudaFree(c->integrated); cudaFree(c->group_counts);
-  sb_frame* fr[] = {c->f_old, c->f_new, c->f_comp, c->cur, c->last, c->cur_model, c->last_model};
-  for (sb_frame* f : fr)
-    if (f) {
-      cudaFree(f->base);
-      delete f;
-    }
-  cudaFree(c->mailbox);
-  cudaFree(c->comm_epoch);
-  cudaFree(c->result_block);
-  return SB_OK;
+// Every write to a frame other than the memoised render itself goes through here: the memo is dropped when it covers
+// the frame (the map's old / new / composed frames, or the `out` frame of the memoised render).
+void frame_written(sb_ctx* c, const sb_frame* f) {
+  if (f == c->f_old || f == c->f_new || f == c->f_comp || f->id == c->memo.key.out) c->memo.clear();
 }
 
 int reset_state(sb_ctx* c) {
   // SurfelMap::reset (SurfelMap.cpp:473-482) + the SurfelMapping members set up in its constructor
-  c->rkey_valid = false;
   c->map_version += 1;
   c->n_host = 0; c->n_updated = 0; c->n_new = 0; c->map_timestamp = 0;
   c->origin_i = c->origin_j = 0;
@@ -293,7 +285,7 @@ int reset_state(sb_ctx* c) {
   c->h_poses_inv = c->h_poses;
   SB_CUDA(c, cudaMemcpyAsync(c->poses, c->h_poses.data(), (size_t)kMaxPoses * 64, cudaMemcpyHostToDevice, c->stream));
   SB_CUDA(c, cudaMemcpyAsync(c->poses_inv, c->h_poses.data(), (size_t)kMaxPoses * 64, cudaMemcpyHostToDevice, c->stream));
-  SB_CUDA(c, cudaMemsetAsync(c->d_counts, 0, 16 * sizeof(uint32_t), c->stream));
+  SB_CUDA(c, cudaMemsetAsync(c->res->counts, 0, sizeof(c->res->counts), c->stream));
   c->timestamp = 0;
   ident_d(c->currentPose); ident_d(c->lastPose); ident_d(c->currentPose_old); ident_d(c->currentPose_new);
   ident_d(c->lastIncrement);
@@ -303,17 +295,16 @@ int reset_state(sb_ctx* c) {
   {
     // staged in the context's own pinned buffer (read by the async copy until the synchronize at the end of this
     // function; no other transfer of this context is in flight here): contexts reset concurrently share nothing
-    static_assert(sizeof(PoseDev) <= 4096, "pinned staging");
-    PoseDev& h = *reinterpret_cast<PoseDev*>(c->h_pinned);
+    PoseDev& h = c->host->result.pose;
     memset(&h, 0, sizeof(h));
     ident_d(h.currentPose); ident_d(h.lastPose); ident_d(h.lastIncrement); ident_d(h.increment); ident_d(h.T0);
     for (int i = 0; i < 4; ++i) h.P_active.m[5 * i] = h.invP_active.m[5 * i] = h.P_cur.m[5 * i] = h.invP_cur.m[5 * i] = 1.0f;
-    SB_CUDA(c, cudaMemcpyAsync(c->pd, &h, sizeof(h), cudaMemcpyHostToDevice, c->stream));
+    SB_CUDA(c, cudaMemcpyAsync(&c->res->pose, &h, sizeof(h), cudaMemcpyHostToDevice, c->stream));
   }
   c->cur_has_semantics = c->last_has_semantics = false;
-  sb_frame* fr[] = {c->f_old, c->f_new, c->f_comp, c->cur, c->last, c->cur_model, c->last_model};
-  for (sb_frame* f : fr)
-    if (f) SB_CUDA(c, cudaMemsetAsync(f->base, 0, (size_t)f->d.W * f->d.H * 3 * sizeof(float4), c->stream));
+  for (const sb_frame* f : {c->f_old.get(), c->f_new.get(), c->f_comp.get(), c->cur.get(), c->last.get(),
+                           c->cur_model.get(), c->last_model.get()})
+    SB_CUDA(c, cudaMemsetAsync(f->base, 0, (size_t)f->d.W * f->d.H * 3 * sizeof(float4), c->stream));
   SB_CUDA(c, cudaStreamSynchronize(c->stream));
   return SB_OK;
 }
@@ -321,79 +312,73 @@ int reset_state(sb_ctx* c) {
 int alloc_buffers(sb_ctx* c) {
   const sb_params& p = c->p;
   size_t Pd = (size_t)p.data_width * p.data_height, Pm = (size_t)p.model_width * p.model_height;
-  // the per-scan results live in ONE device block with the layout of the pinned host mirror, so that the end of a scan is
-  // a single device-to-host copy: [0] PoseDev, [4096] 64 int64 statistics sums, [8192] 16 uint32 surfel counts
-  static_assert(sizeof(PoseDev) <= 4096, "PoseDev must fit the first page of the result block");
-  SB_CUDA(c, cudaMalloc(&c->result_block, 8192 + 64));
-  SB_CUDA(c, cudaMemsetAsync(c->result_block, 0, 8192 + 64, c->stream));
-  c->pd = reinterpret_cast<PoseDev*>(c->result_block);
-  c->acc32 = reinterpret_cast<long long*>(c->result_block + 4096);
-  c->d_counts = reinterpret_cast<uint32_t*>(c->result_block + 8192);
+  SB_CUDA(c, dev_alloc(c->res, sizeof(ResultBlock)));
+  SB_CUDA(c, cudaMemsetAsync(c->res, 0, sizeof(ResultBlock), c->stream));
   const size_t Pk = preprocess_key_elems(p.data_width, p.data_height);
   for (int i = 0; i < 2; ++i) {
-    SB_CUDA(c, cudaMalloc(&c->prep.img[i], Pk * 8));
+    SB_CUDA(c, dev_alloc(c->prep.img[i], Pk * 8));
+    // TMA staging of the key tiles wherever the device has a TMA unit: measured 2 % (64x2048) / 1.5 % (128x4096)
+    // faster than plain loads (DESIGN.md section 4)
     c->prep.tmap_ok[i] = make_key_tensor_map(&c->prep.tmap[i], c->prep.img[i], p.data_width, p.data_height);
   }
-  // TMA staging of the key tiles: measured 2 % (64x2048) / 1.5 % (128x4096) faster than plain loads; SUMA_B200_PREP_TMA=0
-  // selects the plain-load instantiation (DESIGN.md section 4)
-  c->prep.use_tma = true;
-  if (const char* e = getenv("SUMA_B200_PREP_TMA")) c->prep.use_tma = atoi(e) != 0;
   c->pts_cap = Pd * 2 + 1024;
-  SB_CUDA(c, cudaMalloc(&c->d_pts, c->pts_cap * 16));
-  SB_CUDA(c, cudaMalloc(&c->d_labels, c->pts_cap * 4));
-  SB_CUDA(c, cudaMalloc(&c->d_probs, c->pts_cap * 4));
-  SB_CUDA(c, cudaMalloc(&c->gn, sizeof(GnState)));
-  SB_CUDA(c, cudaMalloc(&c->gn2, sizeof(GnState)));
+  SB_CUDA(c, dev_alloc(c->d_pts, c->pts_cap * 16));
+  SB_CUDA(c, dev_alloc(c->d_labels, c->pts_cap * 4));
+  SB_CUDA(c, dev_alloc(c->d_probs, c->pts_cap * 4));
+  SB_CUDA(c, dev_alloc(c->gn, sizeof(GnState)));
+  SB_CUDA(c, dev_alloc(c->gn2, sizeof(GnState)));
   SB_CUDA(c, cudaMemsetAsync(c->gn2, 0, sizeof(GnState), c->stream));
-  SB_CUDA(c, cudaMalloc(&c->acc_slots, 1024 * 32 * sizeof(long long)));
+  SB_CUDA(c, dev_alloc(c->acc_slots, 1024 * 32 * sizeof(long long)));
   SB_CUDA(c, cudaMemsetAsync(c->acc_slots, 0, 1024 * 32 * sizeof(long long), c->stream));
-  SB_CUDA(c, cudaMalloc(&c->ticket, 128));
-  SB_CUDA(c, cudaMalloc(&c->gn_pub, 64 * 8));
+  SB_CUDA(c, dev_alloc(c->ticket, 128));
+  SB_CUDA(c, dev_alloc(c->gn_pub, 64 * 8));
   SB_CUDA(c, cudaMemsetAsync(c->gn_pub, 0, 64 * 8, c->stream));
-  if (const char* e = getenv("SUMA_B200_GN_CACHE")) c->gn_use_cache = atoi(e) != 0;
   SB_CUDA(c, cudaMemsetAsync(c->ticket, 0, 128, c->stream));
-  SB_CUDA(c, cudaMallocHost(&c->h_pinned, 65536));
+  {
+    void* h = nullptr;
+    SB_CUDA(c, cudaMallocHost(&h, sizeof(sb_ctx::Staging)));
+    c->host.reset(static_cast<sb_ctx::Staging*>(h));
+  }
   int r;
-  if ((r = alloc_planes(c, &c->A, kMaxSurfels))) return r;
-  if ((r = alloc_planes(c, &c->T, kMaxSurfels))) return r;
-  if ((r = alloc_planes(c, &c->G, Pd))) return r;
-  if ((r = alloc_planes(c, &c->X, 16))) return r;
-  if ((r = alloc_planes(c, &c->pool, kTilePoolCap))) return r;
-  SB_CUDA(c, cudaMalloc(&c->d_pool_top, 64));
-  SB_CUDA(c, cudaMalloc(&c->d_tile_rec, (size_t)kMaxTileSlots * sizeof(uint2)));
-  SB_CUDA(c, cudaMalloc(&c->keep, kMaxSurfels));
+  if ((r = alloc_planes(c, c->A_mem, &c->A, kMaxSurfels))) return r;
+  if ((r = alloc_planes(c, c->T_mem, &c->T, kMaxSurfels))) return r;
+  if ((r = alloc_planes(c, c->G_mem, &c->G, Pd))) return r;
+  if ((r = alloc_planes(c, c->X_mem, &c->X, 16))) return r;
+  if ((r = alloc_planes(c, c->pool_mem, &c->pool, kTilePoolCap))) return r;
+  SB_CUDA(c, dev_alloc(c->d_pool_top, 64));
+  SB_CUDA(c, dev_alloc(c->d_tile_rec, (size_t)kMaxTileSlots * sizeof(uint2)));
+  SB_CUDA(c, dev_alloc(c->keep, kMaxSurfels));
   size_t nb = (kMaxSurfels + 127) / 128 + 16;  // blocks of the finest-grained surfel kernel
-  SB_CUDA(c, cudaMalloc(&c->block_counts, nb * 4));
-  SB_CUDA(c, cudaMalloc(&c->block_offsets, nb * 4));
-  SB_CUDA(c, cudaMalloc(&c->lb_desc, (nb + 16) * 8));
+  SB_CUDA(c, dev_alloc(c->block_counts, nb * 4));
+  SB_CUDA(c, dev_alloc(c->block_offsets, nb * 4));
+  SB_CUDA(c, dev_alloc(c->lb_desc, (nb + 16) * 8));
   SB_CUDA(c, cudaMemsetAsync(c->lb_desc, 0, (nb + 16) * 8, c->stream));
-  SB_CUDA(c, cudaMalloc(&c->lb_ticket, 64));
+  SB_CUDA(c, dev_alloc(c->lb_ticket, 64));
   SB_CUDA(c, cudaMemsetAsync(c->lb_ticket, 0, 64, c->stream));
-  SB_CUDA(c, cudaMalloc(&c->poses, (size_t)kMaxPoses * 64));
-  SB_CUDA(c, cudaMalloc(&c->poses_inv, (size_t)kMaxPoses * 64));
-  SB_CUDA(c, cudaMalloc(&c->Mtab_old, (size_t)kMaxPoses * 64));
-  SB_CUDA(c, cudaMalloc(&c->Mtab_new, (size_t)kMaxPoses * 64));
-  SB_CUDA(c, cudaMalloc(&c->key_old, Pm * 8 * 3));
+  SB_CUDA(c, dev_alloc(c->poses, (size_t)kMaxPoses * 64));
+  SB_CUDA(c, dev_alloc(c->poses_inv, (size_t)kMaxPoses * 64));
+  SB_CUDA(c, dev_alloc(c->Mtab_old, (size_t)kMaxPoses * 64));
+  SB_CUDA(c, dev_alloc(c->Mtab_new, (size_t)kMaxPoses * 64));
+  SB_CUDA(c, dev_alloc(c->key_old, Pm * 8 * 3));
   c->key_new = c->key_old + Pm;
   c->key_comp = c->key_old + 2 * Pm;
   SB_CUDA(c, cudaMemsetAsync(c->key_old, 0xff, Pm * 8 * 3, c->stream));
-  for (int i = 0; i < 2; ++i)
-    SB_CUDA(c, cudaMemsetAsync(c->prep.img[i], 0xff, preprocess_key_elems(c->p.data_width, c->p.data_height) * 8, c->stream));
+  for (int i = 0; i < 2; ++i) SB_CUDA(c, cudaMemsetAsync(c->prep.img[i], 0xff, Pk * 8, c->stream));
   c->prep.cur = 0;
-  SB_CUDA(c, cudaMalloc(&c->key_index, Pd * 8));
-  SB_CUDA(c, cudaMalloc(&c->radius_map, Pd * 16));
-  SB_CUDA(c, cudaMalloc(&c->integrated, Pd));
-  SB_CUDA(c, cudaMalloc(&c->group_counts, kGroupCounts * 4));
+  SB_CUDA(c, dev_alloc(c->key_index, Pd * 8));
+  SB_CUDA(c, dev_alloc(c->radius_map, Pd * 16));
+  SB_CUDA(c, dev_alloc(c->integrated, Pd));
+  SB_CUDA(c, dev_alloc(c->group_counts, kGroupCounts * 4));
   SB_CUDA(c, cudaMemsetAsync(c->group_counts, 0, kGroupCounts * 4, c->stream));
-  SB_CUDA(c, cudaMalloc(&c->comm_epoch, 64));
+  SB_CUDA(c, dev_alloc(c->comm_epoch, 64));
   SB_CUDA(c, cudaMemsetAsync(c->comm_epoch, 0, 64, c->stream));
-  if ((r = frame_create(c, p.model_width, p.model_height, &c->f_old))) return r;
-  if ((r = frame_create(c, p.model_width, p.model_height, &c->f_new))) return r;
-  if ((r = frame_create(c, p.model_width, p.model_height, &c->f_comp))) return r;
-  if ((r = frame_create(c, p.data_width, p.data_height, &c->cur))) return r;
-  if ((r = frame_create(c, p.data_width, p.data_height, &c->last))) return r;
-  if ((r = frame_create(c, p.model_width, p.model_height, &c->cur_model))) return r;
-  if ((r = frame_create(c, p.model_width, p.model_height, &c->last_model))) return r;
+  if ((r = frame_create(c, p.model_width, p.model_height, c->f_old))) return r;
+  if ((r = frame_create(c, p.model_width, p.model_height, c->f_new))) return r;
+  if ((r = frame_create(c, p.model_width, p.model_height, c->f_comp))) return r;
+  if ((r = frame_create(c, p.data_width, p.data_height, c->cur))) return r;
+  if ((r = frame_create(c, p.data_width, p.data_height, c->last))) return r;
+  if ((r = frame_create(c, p.model_width, p.model_height, c->cur_model))) return r;
+  if ((r = frame_create(c, p.model_width, p.model_height, c->last_model))) return r;
   return reset_state(c);
 }
 
@@ -427,12 +412,22 @@ FrameDev null_frame() {
   return f;
 }
 
+sb_ctx::RenderMemo::Key memo_key(const sb_ctx* c, const float* pose_old, const float* pose_new, float conf_thr,
+                                 const sb_frame* out) {
+  sb_ctx::RenderMemo::Key k{};
+  memcpy(k.pose_old, pose_old, 64);
+  memcpy(k.pose_new, pose_new, 64);
+  k.conf_thr = conf_thr;
+  k.map_timestamp = c->map_timestamp;
+  k.map_version = c->map_version;
+  k.out = out->id;
+  k.compose = c->p.compose_rendering;
+  return k;
+}
+
 int render_full(sb_ctx* c, const float* pose_old, const float* pose_new, float conf_thr, sb_frame* out,
                 const Mat4* inv_dev = nullptr, bool table_ready = false) {
-  if (!inv_dev && c->rkey_valid && c->rkey.out == out && c->rkey.map_version == c->map_version &&
-      c->rkey.map_timestamp == c->map_timestamp && c->rkey.compose == c->p.compose_rendering &&
-      memcmp(&c->rkey.conf_thr, &conf_thr, 4) == 0 && memcmp(c->rkey.pose_old, pose_old, 64) == 0 &&
-      memcmp(c->rkey.pose_new, pose_new, 64) == 0) {
+  if (!inv_dev && c->memo.matches(memo_key(c, pose_old, pose_new, conf_thr, out))) {
     c->renders_skipped += 1;  // old / new / composed frames and `out` already hold exactly this rendering
     return SB_OK;
   }
@@ -459,41 +454,34 @@ int render_full(sb_ctx* c, const float* pose_old, const float* pose_new, float c
     RenderTargets t{c->key_old, c->key_new, nullptr};
     int thr = t_threshold(c);
     if (same) {
-      launch_render_scatter(L, kp, c->A, c->d_counts, n_grid(c), c->Mtab_old, conf_thr, thr, 1, 1, 0, t);
+      launch_render_scatter(L, kp, c->A, c->res->counts, n_grid(c), c->Mtab_old, conf_thr, thr, 1, 1, 0, t);
     } else {
       RenderTargets to{c->key_old, nullptr, nullptr}, tn{nullptr, c->key_new, nullptr};
-      launch_render_scatter(L, kp, c->A, c->d_counts, n_grid(c), c->Mtab_old, conf_thr, thr, 1, 0, 0, to);
-      launch_render_scatter(L, kp, c->A, c->d_counts, n_grid(c), Mnew, conf_thr, thr, 0, 1, 0, tn);
+      launch_render_scatter(L, kp, c->A, c->res->counts, n_grid(c), c->Mtab_old, conf_thr, thr, 1, 0, 0, to);
+      launch_render_scatter(L, kp, c->A, c->res->counts, n_grid(c), Mnew, conf_thr, thr, 0, 1, 0, tn);
     }
     launch_render_resolve(L, kp, c->A, c->Mtab_old, Mnew, t, c->f_old->d, c->f_new->d, c->f_comp->d, out->d, null_frame(), 0, 0);
   } else {
     // SurfelMap.cpp:977-1017: one view with render_old_surfels = false, timestamp_threshold = 0, copied to old and new
     RenderTargets t{nullptr, c->key_new, nullptr};
-    launch_render_scatter(L, kp, c->A, c->d_counts, n_grid(c), c->Mtab_old, conf_thr, 0, 0, 1, 0, t);
+    launch_render_scatter(L, kp, c->A, c->res->counts, n_grid(c), c->Mtab_old, conf_thr, 0, 0, 1, 0, t);
     launch_render_resolve(L, kp, c->A, c->Mtab_old, c->Mtab_old, t, null_frame(), c->f_new->d, null_frame(), null_frame(),
                           null_frame(), 0, 0);
     SB_CUDA(c, cudaMemcpyAsync(c->f_old->base, c->f_new->base, Pm * 48, cudaMemcpyDeviceToDevice, c->stream));
     SB_CUDA(c, cudaMemcpyAsync(out->base, c->f_new->base, Pm * 48, cudaMemcpyDeviceToDevice, c->stream));
   }
-  if (inv_dev) {  // pose still on the device: the caller completes the memo key once it has read the pose back
-    c->rkey_valid = false;
-    return SB_OK;
-  }
-  memcpy(c->rkey.pose_old, pose_old, 64);
-  memcpy(c->rkey.pose_new, pose_new, 64);
-  c->rkey.conf_thr = conf_thr;
-  c->rkey.map_timestamp = c->map_timestamp;
-  c->rkey.map_version = c->map_version;
-  c->rkey.compose = c->p.compose_rendering;
-  c->rkey.out = out;
-  c->rkey_valid = true;
+  if (inv_dev)  // pose still on the device: the caller stores the memo once it has read the pose back
+    c->memo.clear();
+  else
+    c->memo.store(memo_key(c, pose_old, pose_new, conf_thr, out));
   return SB_OK;
 }
 
 // which: 1 = active (new surfels into newMapFrame), 0 = inactive (old surfels into oldMapFrame); Q4: semantic map kept
 int render_single(sb_ctx* c, const float* pose, float conf_thr, int which, const Mat4* inv_dev = nullptr,
                   bool table_ready = false, sb_frame* copy_to = nullptr) {
-  c->rkey_valid = false;  // overwrites vertex / normal of the new (or old) map frame
+  frame_written(c, which ? c->f_new : c->f_old);
+  if (copy_to) frame_written(c, copy_to);
   const KParams& kp = c->kp;
   Launch L = L_(c);
   size_t Pm = (size_t)kp.Wm * kp.Hm;
@@ -502,7 +490,7 @@ int render_single(sb_ctx* c, const float* pose, float conf_thr, int which, const
   if (!table_ready) launch_pose_products(L, mat4_from(inv), inv_dev, c->poses, c->Mtab_old, pose_table_count(c));
   unsigned long long* key = which ? c->key_new : c->key_old;
   RenderTargets t{which ? nullptr : key, which ? key : nullptr, nullptr};
-  launch_render_scatter(L, kp, c->A, c->d_counts, n_grid(c), c->Mtab_old, conf_thr, t_threshold(c), which ? 0 : 1,
+  launch_render_scatter(L, kp, c->A, c->res->counts, n_grid(c), c->Mtab_old, conf_thr, t_threshold(c), which ? 0 : 1,
                         which ? 1 : 0, 0, t);
   // copy_to: lastModelFrame_->copy(*map_->newMapFrame()), SurfelMapping.cpp:407 (the semantic image is the stale one, Q4),
   // written by the same resolve pass
@@ -523,7 +511,7 @@ int render_single(sb_ctx* c, const float* pose, float conf_thr, int which, const
 int gn_fail(sb_ctx* c) {
   cudaMemsetAsync(c->ticket, 0, 128, c->stream);
   cudaMemsetAsync(c->acc_slots, 0, 1024 * 32 * sizeof(long long), c->stream);
-  cudaMemsetAsync(&c->pd->gn_error, 0, sizeof(int), c->stream);
+  cudaMemsetAsync(&c->res->pose.gn_error, 0, sizeof(int), c->stream);
   cudaStreamSynchronize(c->stream);
   return fail(c, SB_ERR_STATE, "Gauss-Newton kernel timed out waiting for a block or a peer GPU");
 }
@@ -544,14 +532,6 @@ IcpArgs icp_args(sb_ctx* c, const sb_frame* data, const sb_frame* model, float m
   a.row_begin = row_begin; a.row_end = row_end;
   a.has_semantics = semantics ? 1 : 0;
   a.Wm = model->d.W; a.Hm = model->d.H;
-  {  // stride ~ 0.618 * rows, coprime to rows
-    int rows = row_end - row_begin;
-    int step = (int)(rows * 0.6180339887) | 1;
-    auto gcd = [](int x, int y) { while (y) { int t = x % y; x = y; y = t; } return x; };
-    while (rows > 1 && gcd(step, rows) != 1) step += 2;
-    a.row_step = rows > 1 ? step % rows : 1;
-    if (a.row_step == 0) a.row_step = 1;
-  }
   return a;
 }
 
@@ -570,46 +550,34 @@ int icp_jacobian_raw(sb_ctx* c, const sb_frame* data, const sb_frame* model, con
   IcpArgs a = icp_args(c, data, model, max_distance, max_angle_deg, r0, r1, semantics);
   Mat4 P;
   for (int i = 0; i < 16; ++i) P.m[i] = (float)pose[i];  // pose_.cast<float>(), Frame2Model.cpp:194
-  launch_icp_jacobian(L_(c), c->kp, a, P, iteration, c->acc32, c->acc_slots, c->ticket + 16, c->icp_blocks);
-  SB_CUDA(c, cudaMemcpyAsync(c->h_pinned, c->acc32, 32 * sizeof(long long), cudaMemcpyDeviceToHost, c->stream));
+  launch_icp_jacobian(L_(c), c->kp, a, P, iteration, c->res->sums, c->acc_slots, c->ticket + 16, c->icp_blocks);
+  SB_CUDA(c, cudaMemcpyAsync(c->host->sums, c->res->sums, sizeof(c->host->sums), cudaMemcpyDeviceToHost, c->stream));
   SB_CUDA(c, cudaStreamSynchronize(c->stream));
-  memcpy(raw, c->h_pinned, 32 * sizeof(long long));
+  memcpy(raw, c->host->sums, sizeof(c->host->sums));
   return SB_OK;
 }
 
-// enqueue the device-resident Gauss-Newton loop; the result stays in c->gn
-struct GnHead {  // prefix of GnState copied back / uploaded
-  double pose[16];
-  double last_error;
-  double out48[48];
-  int k, done, history_len, error;
-};
-
-// Row-striped minimisation with a host-side all-reduce callback: LieGaussNewton::minimize driven from the host, one
-// striped K5 launch + 256-byte read-back + callback per iteration; the result is written into the device GN state so
-// that the rest of the pipeline proceeds as after the device-resident loop.
-int icp_minimize_callback(sb_ctx* c, const sb_frame* data, const sb_frame* model, const double* T0, int max_iter,
-                          double eps, double delta, float max_distance, float max_angle_deg, bool semantics) {
-  const bool striped = c->comm_cb != nullptr;
-  IcpArgs a = icp_args(c, data, model, max_distance, max_angle_deg, striped ? c->row_begin : 0, striped ? c->row_end : c->kp.H,
-                       semantics);
-  std::vector<double> hist;
-  GnHead h;
+// Row-striped minimisation with a host-side all-reduce callback (sb_comm_set_callback): LieGaussNewton::minimize driven
+// from the host, one striped K5 launch + 256-byte read-back + callback per iteration; the result is written into the
+// device GN state st so that the rest of the pipeline proceeds as after the device-resident loop.
+int icp_minimize_callback(sb_ctx* c, GnState* st, const sb_frame* data, const sb_frame* model, const double* T0,
+                          int max_iter, double eps, double delta, float max_distance, float max_angle_deg, bool semantics) {
+  IcpArgs a = icp_args(c, data, model, max_distance, max_angle_deg, c->row_begin, c->row_end, semantics);
+  GnHead& h = c->host->gn;
   memset(&h, 0, sizeof(h));
   memcpy(h.pose, T0, sizeof(h.pose));
   h.last_error = (double)3.402823466e+38f;
   int k = 0;
   for (;;) {
-    hist.insert(hist.end(), h.pose, h.pose + 16);
+    memcpy(c->host->history + 16 * h.history_len++, h.pose, sizeof(h.pose));  // at most max_iter + 1 <= 257 poses
     if (k >= max_iter) break;
     Mat4 P;
     for (int i = 0; i < 16; ++i) P.m[i] = (float)h.pose[i];
-    launch_icp_jacobian(L_(c), c->kp, a, P, k, c->acc32, c->acc_slots, c->ticket + 16, c->icp_blocks);
-    SB_CUDA(c, cudaMemcpyAsync(c->h_pinned, c->acc32, 32 * sizeof(long long), cudaMemcpyDeviceToHost, c->stream));
+    launch_icp_jacobian(L_(c), c->kp, a, P, k, c->res->sums, c->acc_slots, c->ticket + 16, c->icp_blocks);
+    long long* raw = c->host->sums;
+    SB_CUDA(c, cudaMemcpyAsync(raw, c->res->sums, sizeof(c->host->sums), cudaMemcpyDeviceToHost, c->stream));
     SB_CUDA(c, cudaStreamSynchronize(c->stream));
-    long long raw[32];
-    memcpy(raw, c->h_pinned, sizeof(raw));
-    if (c->comm_cb && c->comm_cb(c->comm_cb_user, (int64_t*)raw) != 0) return fail(c, SB_ERR_STATE, "all-reduce callback failed");
+    if (c->comm_cb(c->comm_cb_user, (int64_t*)raw) != 0) return fail(c, SB_ERR_STATE, "all-reduce callback failed");
     sbg::unpack48(raw, h.out48);
     double dx[6];
     int result = sbg::gn_step(h.out48, h.last_error, eps, delta, h.pose, dx);
@@ -619,74 +587,54 @@ int icp_minimize_callback(sb_ctx* c, const sb_frame* data, const sb_frame* model
   }
   h.k = k;
   h.done = 1;
-  size_t hb = hist.size() * sizeof(double);
-  if (hb > 32768) hb = 32768;  // staging room: 256 poses (a run of all kMaxGnIter = 256 iterations pushes 257)
-  h.history_len = (int)(hb / 128);
-  char* hp = (char*)c->h_pinned + 16384;
-  memcpy(hp, &h, sizeof(h));
-  memcpy(hp + 1024, hist.data(), hb);
-  SB_CUDA(c, cudaMemcpyAsync(c->gn, hp, sizeof(h), cudaMemcpyHostToDevice, c->stream));
-  SB_CUDA(c, cudaMemcpyAsync((char*)c->gn + offsetof(GnState, history), hp + 1024, hb, cudaMemcpyHostToDevice, c->stream));
+  SB_CUDA(c, cudaMemcpyAsync(static_cast<GnHead*>(st), &h, sizeof(h), cudaMemcpyHostToDevice, c->stream));
+  SB_CUDA(c, cudaMemcpyAsync(st->history, c->host->history, (size_t)h.history_len * 16 * sizeof(double),
+                             cudaMemcpyHostToDevice, c->stream));
   SB_CUDA(c, cudaStreamSynchronize(c->stream));
   return SB_OK;
 }
 
+// LieGaussNewton::minimize; the result stays in c->gn. One cooperative launch for the whole minimisation, or the
+// host-driven loop when a host all-reduce callback is set.
 int icp_minimize_enqueue(sb_ctx* c, const sb_frame* data, const sb_frame* model, const double* T0, int max_iter,
                          double eps, double delta, float max_distance, float max_angle_deg, bool semantics) {
   if (max_iter <= 0 || max_iter > kMaxGnIter) max_iter = kMaxGnIter;
-  if (c->comm_cb) return icp_minimize_callback(c, data, model, T0, max_iter, eps, delta, max_distance, max_angle_deg, semantics);
-  int r0 = 0, r1 = c->kp.H;
-  if (c->comm_on) {
-    r0 = c->row_begin;
-    r1 = c->row_end;
-  }
-  if (const char* dr = getenv("SUMA_B200_DEBUG_ROWS")) {  // debugging aid: persistent kernel on a row sub-range
-    int a0 = 0, a1 = 0;
-    if (sscanf(dr, "%d,%d", &a0, &a1) == 2 && a0 >= 0 && a1 <= c->kp.H && a0 < a1) {
-      r0 = a0;
-      r1 = a1;
-    }
-  }
-  IcpArgs a = icp_args(c, data, model, max_distance, max_angle_deg, r0, r1, semantics);
+  if (c->comm_cb)
+    return icp_minimize_callback(c, c->gn, data, model, T0, max_iter, eps, delta, max_distance, max_angle_deg, semantics);
+  IcpArgs a = icp_args(c, data, model, max_distance, max_angle_deg, c->comm_on ? c->row_begin : 0,
+                       c->comm_on ? c->row_end : c->kp.H, semantics);
   Mat4d T;
   memcpy(T.m, T0, sizeof(T.m));
   Launch L = L_(c);
-  if (c->icp_coop_blocks > 0) {
-    // one cooperative launch for the whole minimisation
-    launch_gn_init(L, c->gn, T, c->acc32);
-    GnJob job;
-    memset(&job, 0, sizeof(job));
-    job.mode = GN_PLAIN;
-    job.a = a;
-    job.st = c->gn;
-    job.max_iter = max_iter;
-    job.eps = eps;
-    job.delta = delta;
-    job.epoch_base = next_epoch_base(c, max_iter);
-    job.use_cache = c->gn_use_cache;
-    if (launch_gn_persistent(L, c->kp, job, c->acc_slots, c->ticket, c->gn_pub, c->comm_on ? &c->comm : nullptr,
-                             c->icp_coop_blocks) == 0)
-      return SB_OK;
+  launch_gn_init(L, c->gn, T, c->res->sums);
+  GnJob job;
+  memset(&job, 0, sizeof(job));
+  job.mode = GN_PLAIN;
+  job.a = a;
+  job.st = c->gn;
+  job.max_iter = max_iter;
+  job.eps = eps;
+  job.delta = delta;
+  job.epoch_base = next_epoch_base(c, max_iter);
+  if (launch_gn_persistent(L, c->kp, job, c->acc_slots, c->ticket, c->gn_pub, c->comm_on ? &c->comm : nullptr,
+                           c->icp_coop_blocks) != 0) {
     cudaGetLastError();
-    c->icp_coop_blocks = 0;  // no cooperative launch on this device / context: drive the loop from the host
+    return fail(c, SB_ERR_CUDA, "cooperative launch of the Gauss-Newton kernel failed");
   }
-  if (c->comm_on) return fail(c, SB_ERR_STATE, "the fused peer exchange needs a cooperative launch");
-  return icp_minimize_callback(c, data, model, T0, max_iter, eps, delta, max_distance, max_angle_deg, semantics);
+  return SB_OK;
 }
 
 int icp_minimize_fetch(sb_ctx* c, double* pose_out, double* out48, int* iters, double* history, int* history_len) {
-  SB_CUDA(c, cudaMemcpyAsync(c->h_pinned, c->gn, sizeof(GnHead), cudaMemcpyDeviceToHost, c->stream));
+  GnHead& h = c->host->gn;
+  SB_CUDA(c, cudaMemcpyAsync(&h, static_cast<GnHead*>(c->gn), sizeof(h), cudaMemcpyDeviceToHost, c->stream));
   SB_CUDA(c, cudaStreamSynchronize(c->stream));
-  GnHead h;
-  memcpy(&h, c->h_pinned, sizeof(h));
   if (h.error) return gn_fail(c);
   if (pose_out) memcpy(pose_out, h.pose, sizeof(h.pose));
   if (out48) memcpy(out48, h.out48, sizeof(h.out48));
   if (iters) *iters = h.k;
   if (history_len) *history_len = h.history_len;
   if (history && h.history_len > 0) {
-    SB_CUDA(c, cudaMemcpy(history, (const char*)c->gn + offsetof(GnState, history), (size_t)h.history_len * 128,
-                          cudaMemcpyDeviceToHost));
+    SB_CUDA(c, cudaMemcpy(history, c->gn->history, (size_t)h.history_len * 16 * sizeof(double), cudaMemcpyDeviceToHost));
   }
   return SB_OK;
 }
@@ -699,9 +647,9 @@ float2 submap_center(const sb_ctx* c, int32_t i, int32_t j) {  // submapIndex2ce
 }
 
 int fetch_counts(sb_ctx* c, uint32_t* dst, int n) {
-  SB_CUDA(c, cudaMemcpyAsync(c->h_pinned, c->d_counts, n * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
+  SB_CUDA(c, cudaMemcpyAsync(c->host->result.counts, c->res->counts, n * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
   SB_CUDA(c, cudaStreamSynchronize(c->stream));
-  memcpy(dst, c->h_pinned, n * sizeof(uint32_t));
+  memcpy(dst, c->host->result.counts, n * sizeof(uint32_t));
   return SB_OK;
 }
 
@@ -752,7 +700,8 @@ int append_tiles(sb_ctx* c, int32_t i0, int32_t j0, int di, int dj) {  // Surfel
     appended = true;
   }
   if (appended) {
-    SB_CUDA(c, cudaMemcpyAsync(c->d_counts, &c->n_host, 4, cudaMemcpyHostToDevice, c->stream));
+    c->map_version += 1;
+    SB_CUDA(c, cudaMemcpyAsync(c->res->counts, &c->n_host, 4, cudaMemcpyHostToDevice, c->stream));
     SB_CUDA(c, cudaStreamSynchronize(c->stream));  // the copy reads a member of the context: keep it ordered
   }
   return SB_OK;
@@ -767,7 +716,7 @@ int extract_surfels(sb_ctx* c, bool partially) {
     if (c->n_slots >= kMaxTileSlots) return fail(c, SB_ERR_CAPACITY, "tile cache: out of record slots");
     float2 ctr = submap_center(c, idx.first, idx.second);
     uint32_t slot = c->n_slots++;
-    launch_extract_to_pool(L, c->A, c->d_counts, c->n_host, c->poses, ctr, c->p.submap_extent, c->keep, c->block_counts,
+    launch_extract_to_pool(L, c->A, c->res->counts, c->n_host, c->poses, ctr, c->p.submap_extent, c->keep, c->block_counts,
                            c->block_offsets, c->pool, kTilePoolCap, c->d_pool_top, c->d_tile_rec + slot, kExtractCap);
     DevTile t;
     t.slot = slot;
@@ -828,7 +777,7 @@ int map_update(sb_ctx* c, const float* pose, const sb_frame* frame, const Mat4* 
   // when the frame is the one it produced
   if (!(c->prepped_for_update && frame == c->cur)) launch_radius(L, kp, frame->d, c->radius_map, c->key_index, c->integrated, c->group_counts);
   c->prepped_for_update = false;
-  launch_index_scatter(L, kp, c->A, c->d_counts, n_grid(c), c->Mtab_old, c->key_index);
+  launch_index_scatter(L, kp, c->A, c->res->counts, n_grid(c), c->Mtab_old, c->key_index);
   // K6c + K6e predicate
   float2 ctr = submap_center(c, c->origin_i, c->origin_j);
   float extent = 2.0f * c->p.submap_dimension * c->p.submap_extent + c->p.submap_extent;  // :674
@@ -838,16 +787,16 @@ int map_update(sb_ctx* c, const float* pose, const sb_frame* frame, const Mat4* 
   // with 256-wide windows that stop at the nearest inclusive prefix -- 80.2 us against 48.8 + 23.8 us for the two
   // passes at S = 1.2 M: the ~400 resident blocks finish their heavy per-surfel work together, hold their SM slots
   // through several dependent L2 round trips and only then issue their writes.)
-  launch_update_surfels(L, kp, c->A, c->T, c->d_counts, n_grid(c), mat4_from(pose_h), mat4_from(inv_pose), pose_dev,
+  launch_update_surfels(L, kp, c->A, c->T, c->res->counts, n_grid(c), mat4_from(pose_h), mat4_from(inv_pose), pose_dev,
                         inv_dev, c->poses, c->poses_inv, c->key_index, c->radius_map, frame->d, (int)c->map_timestamp,
                         ctr, extent, c->integrated, c->keep, c->block_counts, c->group_counts);
-  launch_compact_update(L, c->T, c->keep, c->block_counts, c->group_counts, c->d_counts, n_grid(c), c->A, kMaxSurfels,
-                        c->d_counts + 1, c->d_counts + 2);
+  launch_compact_update(L, c->T, c->keep, c->block_counts, c->group_counts, c->res->counts, n_grid(c), c->A, kMaxSurfels,
+                        c->res->counts + 1, c->res->counts + 2);
   // K6d + K6e: new surfels appended behind the updated ones; counts[0] = new map size, counts[3] = new surfels
   c->lb_gen = (c->lb_gen + 1) & 0x3fffffffu;
   if (c->lb_gen == 0) c->lb_gen = 1;
   launch_gen_compact(L, kp, frame->d, c->radius_map, c->integrated, c->poses, (int)c->map_timestamp, ctr, extent, c->A,
-                     c->lb_desc, c->lb_ticket, c->lb_gen, kMaxSurfels, c->d_counts);
+                     c->lb_desc, c->lb_ticket, c->lb_gen, kMaxSurfels, c->res->counts);
   uint64_t up = (uint64_t)n_grid(c) + Pd;  // the map can grow by at most one surfel per pixel
   c->n_upper = up > kMaxSurfels ? kMaxSurfels : (uint32_t)up;
   if (deferred) {
@@ -883,18 +832,16 @@ int grow_point_buffers(sb_ctx* c, size_t n) {
   size_t cap = n + n / 4 + 1024;
   SB_CUDA(c, cudaStreamSynchronize(c->stream));
   if (c->copy_stream) SB_CUDA(c, cudaStreamSynchronize(c->copy_stream));
-  float4* np = nullptr; float* nl = nullptr; float* nq = nullptr;
-  if (cudaMalloc(&np, cap * 16) != cudaSuccess || cudaMalloc(&nl, cap * 4) != cudaSuccess ||
-      cudaMalloc(&nq, cap * 4) != cudaSuccess) {
-    cudaFree(np); cudaFree(nl); cudaFree(nq);
+  DevPtr<float4> np;
+  DevPtr<float> nl, nq;
+  if (dev_alloc(np, cap * 16) != cudaSuccess || dev_alloc(nl, cap * 4) != cudaSuccess ||
+      dev_alloc(nq, cap * 4) != cudaSuccess) {
     cudaGetLastError();
     return fail(c, SB_ERR_CAPACITY, "out of device memory for the scan staging buffers");
   }
-  cudaFree(c->d_pts); cudaFree(c->d_labels); cudaFree(c->d_probs);
-  c->d_pts = np; c->d_labels = nl; c->d_probs = nq;
+  c->d_pts = std::move(np); c->d_labels = std::move(nl); c->d_probs = std::move(nq);
   for (auto& sl : c->prefetch) {  // prefetch slots are re-allocated lazily at the new capacity
-    cudaFree(sl.pts); cudaFree(sl.labels); cudaFree(sl.probs);
-    sl.pts = nullptr; sl.labels = nullptr; sl.probs = nullptr;
+    sl.pts.reset(); sl.labels.reset(); sl.probs.reset();
     sl.valid = false; sl.in_use = false; sl.has_released = false;
   }
   c->pts_cap = cap;
@@ -926,8 +873,8 @@ int upload_scan(sb_ctx* c, const float* pts4, const float* labels, const float* 
       sl.valid = false;
       sl.in_use = true;
       *d_pts = sl.pts;
-      *d_labels = labels ? sl.labels : nullptr;
-      *d_probs = probs ? sl.probs : nullptr;
+      *d_labels = labels ? sl.labels.get() : nullptr;
+      *d_probs = probs ? sl.probs.get() : nullptr;
       return SB_OK;
     }
   }
@@ -935,14 +882,14 @@ int upload_scan(sb_ctx* c, const float* pts4, const float* labels, const float* 
   if (labels && n) SB_CUDA(c, cudaMemcpyAsync(c->d_labels, labels, (size_t)n * 4, cudaMemcpyHostToDevice, c->stream));
   if (probs && n) SB_CUDA(c, cudaMemcpyAsync(c->d_probs, probs, (size_t)n * 4, cudaMemcpyHostToDevice, c->stream));
   *d_pts = c->d_pts;
-  *d_labels = labels ? c->d_labels : nullptr;
-  *d_probs = probs ? c->d_probs : nullptr;
+  *d_labels = labels ? c->d_labels.get() : nullptr;
+  *d_probs = probs ? c->d_probs.get() : nullptr;
   return SB_OK;
 }
 
 // SurfelMap::render_composed, SurfelMap.cpp:1116-1165
 int render_composed_internal(sb_ctx* c, const float* pose_old, const float* pose_new, float conf_thr) {
-  c->rkey_valid = false;
+  frame_written(c, c->f_comp);
   const KParams& kp = c->kp;
   Launch L = L_(c);
   size_t Pm = (size_t)kp.Wm * kp.Hm;
@@ -955,8 +902,8 @@ int render_composed_internal(sb_ctx* c, const float* pose_old, const float* pose
   RenderTargets t{nullptr, nullptr, c->key_comp};
   int thr = t_threshold(c);
   // GL_LEQUAL (SurfelMap.cpp:1126), old then new without clearing (:1146-1152); COLOR2 not attached (Q4)
-  launch_render_scatter(L, kp, c->A, c->d_counts, n_grid(c), c->Mtab_old, conf_thr, thr, 1, 0, 1, t);
-  launch_render_scatter(L, kp, c->A, c->d_counts, n_grid(c), c->Mtab_new, conf_thr, thr, 0, 1, 1, t);
+  launch_render_scatter(L, kp, c->A, c->res->counts, n_grid(c), c->Mtab_old, conf_thr, thr, 1, 0, 1, t);
+  launch_render_scatter(L, kp, c->A, c->res->counts, n_grid(c), c->Mtab_new, conf_thr, thr, 0, 1, 1, t);
   launch_render_resolve(L, kp, c->A, c->Mtab_old, c->Mtab_new, t, null_frame(), null_frame(), c->f_comp->d, null_frame(),
                         null_frame(), 1, 1);
   SB_CUDA(c, cudaGetLastError());
@@ -967,6 +914,7 @@ int render_composed_internal(sb_ctx* c, const float* pose_old, const float* pose
 // recovery minimisation and the pose chaining stay on the device: two cooperative launches (GN_MAIN, GN_POST) around the
 // rendering of the active map at the new pose. Returns with *tables_ready = true when GN_POST has also written the pose
 // table entry of this scan and the table inv(P_cur) * poses[t] (Mtab_old) for the map update / model rendering.
+// With a host all-reduce callback (sb_comm_set_callback) the minimisations are driven from the host instead.
 int update_pose_enqueue(sb_ctx* c, bool* tables_ready) {
   const sb_params& p = c->p;
   const bool sem = c->cur_has_semantics;
@@ -977,14 +925,14 @@ int update_pose_enqueue(sb_ctx* c, bool* tables_ready) {
   int max_iter = p.max_iterations;
   if (max_iter <= 0 || max_iter > kMaxGnIter) max_iter = kMaxGnIter;
   const int r0 = c->comm_on ? c->row_begin : 0, r1 = c->comm_on ? c->row_end : c->kp.H;
-  if (!c->comm_cb && c->icp_coop_blocks > 0) {
+  if (!c->comm_cb) {
     // ---- device-resident path ----
     GnJob job;
     memset(&job, 0, sizeof(job));
     job.mode = GN_MAIN;  // objective_->setData(currentFrame_, map_->newMapFrame()); gn_->minimize(*objective_, T0)   :384-389
     job.a = icp_args(c, c->cur, c->f_new, p.icp_max_distance, p.icp_max_angle, r0, r1, sem);
     job.st = c->gn;
-    job.pd = c->pd;
+    job.pd = &c->res->pose;
     job.Mtab = c->Mtab_old;
     job.poses = c->poses;
     job.n_poses = np;
@@ -995,14 +943,13 @@ int update_pose_enqueue(sb_ctx* c, bool* tables_ready) {
     job.eps = p.stopping_threshold;
     job.delta = p.delta;
     job.epoch_base = next_epoch_base(c, max_iter);
-    job.use_cache = c->gn_use_cache;
     if (launch_gn_persistent(L, c->kp, job, c->acc_slots, c->ticket, c->gn_pub, c->comm_on ? &c->comm : nullptr,
                              c->icp_coop_blocks) != 0) {
       cudaGetLastError();
       return fail(c, SB_ERR_CUDA, "cooperative launch of the Gauss-Newton kernel failed");
     }
     // :405-413: render_active at the new pose (its product table is ready), copied into lastModelFrame_
-    if ((r = render_single(c, nullptr, conf_threshold(c), 1, &c->pd->invP_active, true, c->last_model))) return r;
+    if ((r = render_single(c, nullptr, conf_threshold(c), 1, &c->res->pose.invP_active, true, c->last_model))) return r;
     // :414-449: statistics pass at identity, track-loss recovery, pose chaining, pose-table entry, table for the update
     GnJob post;
     memset(&post, 0, sizeof(post));
@@ -1011,8 +958,8 @@ int update_pose_enqueue(sb_ctx* c, bool* tables_ready) {
     post.fb = icp_args(c, c->cur, c->last, p.fallback_max_distance, p.fallback_max_angle, r0, r1,
                        sem && c->last_has_semantics);
     post.st = c->gn2;
-    post.pd = c->pd;
-    post.stats32 = c->acc32;
+    post.pd = &c->res->pose;
+    post.stats32 = c->res->sums;
     post.poses = c->poses;
     post.poses_inv = c->poses_inv;
     post.t_map = c->map_timestamp;
@@ -1024,7 +971,6 @@ int update_pose_enqueue(sb_ctx* c, bool* tables_ready) {
     post.eps = p.stopping_threshold;
     post.delta = p.delta;
     post.epoch_base = next_epoch_base(c, max_iter);
-    post.use_cache = 0;
     if (launch_gn_persistent(L, c->kp, post, c->acc_slots, c->ticket, c->gn_pub, c->comm_on ? &c->comm : nullptr,
                              c->icp_coop_blocks) != 0) {
       cudaGetLastError();
@@ -1033,7 +979,7 @@ int update_pose_enqueue(sb_ctx* c, bool* tables_ready) {
     *tables_ready = true;
     return SB_OK;
   }
-  // ---- host-driven path (all-reduce callback, or no cooperative launch): the round-1 sequence of small launches ----
+  // ---- host-driven path (all-reduce callback): one Jacobian launch and one callback per iteration ----
   double T0[16];
   if (!p.initialize_identity) memcpy(T0, c->lastIncrement, sizeof(T0)); else ident_d(T0);
   if ((r = icp_minimize_enqueue(c, c->cur, c->f_new, T0, p.max_iterations, p.stopping_threshold, p.delta,
@@ -1041,30 +987,25 @@ int update_pose_enqueue(sb_ctx* c, bool* tables_ready) {
     return r;
   Mat4d T0v;
   memcpy(T0v.m, T0, sizeof(T0v.m));
-  launch_pose_after_icp(L, c->gn, c->pd, T0v, c->timestamp, p.fallback_mode);
-  if ((r = render_single(c, nullptr, conf_threshold(c), 1, &c->pd->invP_active, false, c->last_model))) return r;
+  launch_pose_after_icp(L, c->gn, &c->res->pose, T0v, c->timestamp, p.fallback_mode);
+  if ((r = render_single(c, nullptr, conf_threshold(c), 1, &c->res->pose.invP_active, false, c->last_model))) return r;
   {
     IcpArgs a = icp_args(c, c->cur, c->f_new, p.icp_max_distance, p.icp_max_angle, 0, c->kp.H, sem);
     Mat4 I;
     for (int i = 0; i < 16; ++i) I.m[i] = (i % 5 == 0) ? 1.0f : 0.0f;
-    launch_icp_jacobian(L, c->kp, a, I, 0, c->acc32, c->acc_slots, c->ticket + 16, c->icp_blocks);
+    launch_icp_jacobian(L, c->kp, a, I, 0, c->res->sums, c->acc_slots, c->ticket + 16, c->icp_blocks);
   }
   if (p.fallback_mode) {  // read the track-loss flag and run the recovery minimisation only when it is set
-    int fb = 0;
-    SB_CUDA(c, cudaMemcpyAsync(c->h_pinned, (const char*)c->pd + offsetof(PoseDev, fallback), sizeof(int),
-                               cudaMemcpyDeviceToHost, c->stream));
+    int& fb = c->host->result.pose.fallback;
+    SB_CUDA(c, cudaMemcpyAsync(&fb, &c->res->pose.fallback, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
     SB_CUDA(c, cudaStreamSynchronize(c->stream));
-    memcpy(&fb, c->h_pinned, sizeof(int));
     if (fb) {
-      GnState* keep = c->gn;
-      c->gn = c->gn2;  // icp_minimize_callback writes its result into c->gn
-      int rr = icp_minimize_callback(c, c->cur, c->last, T0, max_iter, p.stopping_threshold, p.delta,
-                                     p.fallback_max_distance, p.fallback_max_angle, sem && c->last_has_semantics);
-      c->gn = keep;
-      if (rr) return rr;
+      if ((r = icp_minimize_callback(c, c->gn2, c->cur, c->last, T0, max_iter, p.stopping_threshold, p.delta,
+                                     p.fallback_max_distance, p.fallback_max_angle, sem && c->last_has_semantics)))
+        return r;
     }
   }
-  launch_pose_finalize(L, c->gn2, c->pd, 1, c->poses, c->poses_inv, c->map_timestamp);
+  launch_pose_finalize(L, c->gn2, &c->res->pose, 1, c->poses, c->poses_inv, c->map_timestamp);
   return SB_OK;
 }
 
@@ -1101,7 +1042,8 @@ struct CudaLoopBackend {
 };
 
 // host copy of the device-resident pose block after updatePose (shared by the end of every scan and the loop-closure step)
-void absorb_pose_block(sb_ctx* c, const PoseDev& pdh, const char* hp, bool had_icp) {
+void absorb_pose_block(sb_ctx* c, const ResultBlock& rb, bool had_icp) {
+  const PoseDev& pdh = rb.pose;
   memcpy(c->lastPose, pdh.lastPose, sizeof(c->lastPose));
   memcpy(c->currentPose, pdh.currentPose, sizeof(c->currentPose));
   memcpy(c->lastPose_old, c->currentPose_old, sizeof(c->lastPose_old));  // lastPose_old_ = currentPose_old_   :454
@@ -1110,10 +1052,8 @@ void absorb_pose_block(sb_ctx* c, const PoseDev& pdh, const char* hp, bool had_i
   memcpy(c->lastIncrement, pdh.lastIncrement, sizeof(c->lastIncrement));
   c->trackLoss = (uint32_t)pdh.trackLoss;
   if (had_icp) {
-    long long raw[32];
     double r48[48];
-    memcpy(raw, hp + 4096, sizeof(raw));
-    sbg::unpack48(raw, r48);
+    sbg::unpack48(rb.sums, r48);
     c->stats[0] = pdh.icp_iterations;
     c->stats[1] = r48[43];
     c->stats[3] = r48[44];
@@ -1137,15 +1077,11 @@ void absorb_pose_block(sb_ctx* c, const PoseDev& pdh, const char* hp, bool had_i
 int loop_closure_step(sb_ctx* c) {
   namespace lp = suma_b200::loop;
   if (c->comm_on || c->comm_cb) return fail(c, SB_ERR_STATE, "loop closure is not available in row-striped multi-GPU mode");
-  char* hp = (char*)c->h_pinned;
-  SB_CUDA(c, cudaMemcpyAsync(hp, c->result_block, 8192 + 64, cudaMemcpyDeviceToHost, c->stream));
-  const double t_enqueued = now_s();
+  const ResultBlock& rb = c->host->result;
+  SB_CUDA(c, cudaMemcpyAsync(&c->host->result, c->res, sizeof(ResultBlock), cudaMemcpyDeviceToHost, c->stream));
   SB_CUDA(c, cudaStreamSynchronize(c->stream));
-  const double t_synced = now_s();
-  PoseDev pdh;
-  memcpy(&pdh, hp, sizeof(pdh));
-  if (pdh.gn_error) return gn_fail(c);
-  absorb_pose_block(c, pdh, hp, true);
+  if (rb.pose.gn_error) return gn_fail(c);
+  absorb_pose_block(c, rb, true);
   lp::Poses P;
   memcpy(P.current.m, c->currentPose, 128);
   memcpy(P.current_old.m, c->currentPose_old, 128);
@@ -1153,7 +1089,7 @@ int loop_closure_step(sb_ctx* c) {
   memcpy(P.last_old.m, c->lastPose_old, 128);
   memcpy(P.last_increment.m, c->lastIncrement, 128);
   lp::M4 inc;
-  memcpy(inc.m, pdh.increment, 128);
+  memcpy(inc.m, rb.pose.increment, 128);
   c->loop.after_update_pose(c->timestamp, inc, P.current);
   CudaLoopBackend be{c};
   lp::check_loop_closure(c->loop, be, c->timestamp, P);
@@ -1225,17 +1161,17 @@ int sb_create(const sb_params* p, int device, sb_ctx** out) {
   if (cudaGetDeviceProperties(&prop, device) == cudaSuccess) c->sm_count = prop.multiProcessorCount;
   c->icp_blocks = icp_grid_blocks(c->sm_count);
   {
+    // the Gauss-Newton loop is one cooperative launch (the host all-reduce callback aside): no device without it
     int coop = 0;
     cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, device);
     int maxb = coop ? gn_persistent_max_blocks(c->sm_count) : 0;
-    c->icp_coop_blocks = maxb < c->icp_blocks ? maxb : c->icp_blocks;
-    if (c->icp_coop_blocks > 0) c->icp_coop_blocks = icp_balanced_blocks(p->data_width * p->data_height, c->icp_coop_blocks);
-    c->icp_blocks = icp_balanced_blocks(p->data_width * p->data_height, c->icp_blocks);
-    if (getenv("SUMA_B200_NO_PERSISTENT_GN")) c->icp_coop_blocks = 0;
-    if (getenv("SUMA_B200_ICP_BLOCKS")) {
-      int b = atoi(getenv("SUMA_B200_ICP_BLOCKS"));
-      if (b > 0 && b <= maxb && b <= 1024) c->icp_coop_blocks = b;
+    if (maxb <= 0) {
+      fprintf(stderr, "sb_create: device %d cannot run the cooperative Gauss-Newton kernel\n", device);
+      delete c;
+      return SB_ERR_CUDA;
     }
+    c->icp_coop_blocks = icp_balanced_blocks(p->data_width * p->data_height, maxb < c->icp_blocks ? maxb : c->icp_blocks);
+    c->icp_blocks = icp_balanced_blocks(p->data_width * p->data_height, c->icp_blocks);
   }
   if (cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking) != cudaSuccess) {
     delete c;
@@ -1245,7 +1181,6 @@ int sb_create(const sb_params* p, int device, sb_ctx** out) {
   int r = alloc_buffers(c);
   if (r != SB_OK) {
     fprintf(stderr, "sb_create: %s\n", c->err.c_str());
-    release_buffers(c);
     cudaStreamDestroy(c->stream);
     delete c;
     return r;
@@ -1259,9 +1194,7 @@ int sb_destroy(sb_ctx* c) {
   cudaSetDevice(c->device);
   cudaStreamSynchronize(c->stream);
   sb_comm_shutdown(c);
-  release_buffers(c);
   for (auto& sl : c->prefetch) {
-    cudaFree(sl.pts); cudaFree(sl.labels); cudaFree(sl.probs);
     if (sl.done) cudaEventDestroy(sl.done);
     if (sl.released) cudaEventDestroy(sl.released);
   }
@@ -1272,7 +1205,7 @@ int sb_destroy(sb_ctx* c) {
   }
   for (cudaEvent_t e : c->prof.pool) cudaEventDestroy(e);
   cudaStreamDestroy(c->stream);
-  delete c;
+  delete c;  // frees the context's device and pinned memory
   return SB_OK;
 }
 
@@ -1289,7 +1222,7 @@ int sb_set_params(sb_ctx* c, const sb_params* p) {
     return fail(c, SB_ERR_STATE, "set_params: image sizes are fixed at sb_create (as in SurfelMapping's constructor)");
   c->p = *p;
   derive(c);
-  c->rkey_valid = false;
+  c->memo.clear();
   return SB_OK;
 }
 
@@ -1305,21 +1238,25 @@ void* sb_stream(sb_ctx* c) { return c ? (void*)c->stream : nullptr; }
 uint64_t sb_launch_count(const sb_ctx* c) { return c ? c->launches : 0; }
 
 int sb_frame_create(sb_ctx* c, int w, int h, sb_frame** out) {
-  if (!c) return SB_ERR_INVALID;
+  if (!c || !out) return fail(c, SB_ERR_INVALID, "frame_create: bad arguments");
   cudaSetDevice(c->device);
-  return frame_create(c, w, h, out);
+  FramePtr f;
+  int r = frame_create(c, w, h, f);
+  if (r) return r;
+  *out = f.release();
+  return SB_OK;
 }
 int sb_frame_destroy(sb_frame* f) {
   if (!f) return SB_ERR_INVALID;
   cudaStreamSynchronize(f->ctx->stream);
-  cudaFree(f->base);
+  frame_written(f->ctx, f);
   delete f;
   return SB_OK;
 }
 int sb_frame_copy(sb_frame* dst, const sb_frame* src) {
   if (!dst || !src || dst->d.W != src->d.W || dst->d.H != src->d.H) return SB_ERR_INVALID;
   sb_ctx* c = dst->ctx;
-  c->rkey_valid = false;
+  frame_written(c, dst);
   SB_CUDA(c, cudaMemcpyAsync(dst->base, src->base, (size_t)src->d.W * src->d.H * 48, cudaMemcpyDeviceToDevice, c->stream));
   return SB_OK;
 }
@@ -1336,7 +1273,7 @@ int sb_frame_download(const sb_frame* f, int which, float* dst) {
 int sb_frame_upload(sb_frame* f, int which, const float* src) {
   if (!f || !src || which < 0 || which > 2) return SB_ERR_INVALID;
   sb_ctx* c = f->ctx;
-  c->rkey_valid = false;
+  frame_written(c, f);
   SB_CUDA(c, cudaMemcpyAsync(frame_plane(f, which), src, (size_t)f->d.W * f->d.H * 16, cudaMemcpyHostToDevice, c->stream));
   SB_CUDA(c, cudaStreamSynchronize(c->stream));
   return SB_OK;
@@ -1356,6 +1293,7 @@ int sb_preprocess(sb_ctx* c, const float* pts4, const float* labels, const float
   const float4* dp; const float* dl; const float* dq;
   int r = upload_scan(c, pts4, labels, probs, n, on_device, &dp, &dl, &dq);
   if (r) return r;
+  frame_written(c, out);
   launch_preprocess(L_(c), c->kp, dp, dl, dq, n, timestamp, c->prep, out->d, nullptr, nullptr, nullptr, nullptr);
   SB_CUDA(c, cudaGetLastError());
   return SB_OK;
@@ -1529,7 +1467,7 @@ int sb_map_upload(sb_ctx* c, const sb_surfel* src, uint32_t n, uint32_t timestam
   c->n_upper = n;
   c->map_timestamp = timestamp;
   c->map_version += 1;
-  SB_CUDA(c, cudaMemcpyAsync(c->d_counts, &c->n_host, 4, cudaMemcpyHostToDevice, c->stream));
+  SB_CUDA(c, cudaMemcpyAsync(c->res->counts, &c->n_host, 4, cudaMemcpyHostToDevice, c->stream));
   SB_CUDA(c, cudaStreamSynchronize(c->stream));
   return SB_OK;
 }
@@ -1575,6 +1513,7 @@ int sb_process_scan(sb_ctx* c, const float* pts4, const float* labels, const flo
   c->cur_has_semantics = labels != nullptr;
   // ---- everything below is enqueued on the stream without a host round trip; ONE synchronisation at the end ----
   // preprocess(), :342-358
+  frame_written(c, c->cur);
   launch_preprocess(L, c->kp, dp, dl, dq, n, c->timestamp, c->prep, c->cur->d, c->radius_map, c->key_index, c->integrated,
                     c->group_counts);
   c->prepped_for_update = true;
@@ -1594,57 +1533,41 @@ int sb_process_scan(sb_ctx* c, const float* pts4, const float* labels, const flo
       loop_ran = true;
     }
   } else {
-    launch_pose_finalize(L, c->gn2, c->pd, 0, c->poses, c->poses_inv, c->map_timestamp);
+    launch_pose_finalize(L, c->gn2, &c->res->pose, 0, c->poses, c->poses_inv, c->map_timestamp);
   }
   // updateMap(), :797-804
   const uint32_t t_map = c->map_timestamp;
-  if ((r = map_update(c, nullptr, c->cur, &c->pd->P_cur, &c->pd->invP_cur, tables_ready))) return r;
+  if ((r = map_update(c, nullptr, c->cur, &c->res->pose.P_cur, &c->res->pose.invP_cur, tables_ready))) return r;
   float ct2 = conf_threshold(c);
   if (p.render_after_update) {
-    if ((r = render_full(c, nullptr, nullptr, ct2, c->cur_model, &c->pd->invP_cur, true))) return r;
+    if ((r = render_full(c, nullptr, nullptr, ct2, c->cur_model, &c->res->pose.invP_cur, true))) return r;
   }
   // ---- the scan's results: pose block, statistics sums, surfel counts ----
-  char* hp = (char*)c->h_pinned;
-  SB_CUDA(c, cudaMemcpyAsync(hp, c->result_block, 8192 + 64, cudaMemcpyDeviceToHost, c->stream));
+  const ResultBlock& rb = c->host->result;
+  SB_CUDA(c, cudaMemcpyAsync(&c->host->result, c->res, sizeof(ResultBlock), cudaMemcpyDeviceToHost, c->stream));
   const double t_enqueued = now_s();
   SB_CUDA(c, cudaStreamSynchronize(c->stream));
   const double t_synced = now_s();
   SB_CUDA(c, cudaGetLastError());
-  PoseDev pdh;
-  memcpy(&pdh, hp, sizeof(pdh));
-  if (pdh.gn_error) return gn_fail(c);
-  if (!loop_ran) absorb_pose_block(c, pdh, hp, had_icp);  // (the loop-closure step has already done it, and chose currentPose_old_)
-  uint32_t cnt[4];
-  memcpy(cnt, hp + 8192, sizeof(cnt));
-  c->n_host = cnt[0];
-  c->n_upper = cnt[0];
-  c->n_updated = cnt[2];
-  c->n_new = cnt[3];
+  if (rb.pose.gn_error) return gn_fail(c);
+  if (!loop_ran) absorb_pose_block(c, rb, had_icp);  // (the loop-closure step has already done it, and chose currentPose_old_)
+  c->n_host = rb.counts[0];
+  c->n_upper = rb.counts[0];
+  c->n_updated = rb.counts[2];
+  c->n_new = rb.counts[3];
+  const Mat4 P_cur = rb.pose.P_cur;
   if (t_map < kMaxPoses) {  // host mirror of the pose table entry written by k_pose_finalize
-    memcpy(&c->h_poses[16 * (size_t)t_map], pdh.P_cur.m, 64);
-    sbg::rigid_inverse_f(pdh.P_cur.m, &c->h_poses_inv[16 * (size_t)t_map]);
+    memcpy(&c->h_poses[16 * (size_t)t_map], P_cur.m, 64);
+    sbg::rigid_inverse_f(P_cur.m, &c->h_poses_inv[16 * (size_t)t_map]);
   }
-  if (p.render_after_update) {  // complete the render memo now that the pose bits are known on the host
-    memcpy(c->rkey.pose_old, pdh.P_cur.m, 64);
-    memcpy(c->rkey.pose_new, pdh.P_cur.m, 64);
-    c->rkey.conf_thr = ct2;
-    c->rkey.map_timestamp = c->map_timestamp;
-    c->rkey.map_version = c->map_version;
-    c->rkey.compose = c->p.compose_rendering;
-    c->rkey.out = c->cur_model;
-    c->rkey_valid = true;
-  }
+  if (p.render_after_update)  // the render's memo entry, now that the pose bits are known on the host
+    c->memo.store(memo_key(c, P_cur.m, P_cur.m, ct2, c->cur_model));
   // submap paging (SurfelMap.cpp:547, 744-824) with the pose now known on the host. Re-inserting cached tiles changes
   // the map after the model was rendered: render again in that (rare) case, as the reference renders after paging.
   {
-    const uint64_t v0 = c->map_version;
     const uint32_t n0 = c->n_host;
-    if ((r = update_active_submaps(c, pdh.P_cur.m))) return r;
-    if (c->n_host != n0) {
-      c->map_version = v0 + 1;
-      c->rkey_valid = false;
-      if (p.render_after_update && (r = render_full(c, pdh.P_cur.m, pdh.P_cur.m, ct2, c->cur_model))) return r;
-    }
+    if ((r = update_active_submaps(c, P_cur.m))) return r;
+    if (c->n_host != n0 && p.render_after_update && (r = render_full(c, P_cur.m, P_cur.m, ct2, c->cur_model))) return r;
   }
   c->stats[7] = c->n_host;
   // The reference's three stage timers (preprocessing / icp / mapping) have no meaning here -- the stages overlap on
@@ -1676,9 +1599,9 @@ int sb_prefetch_scan(sb_ctx* c, const float* pts4, const float* labels, const fl
   }
   for (auto& sl : c->prefetch)
     if (!sl.pts) {  // first use, or the staging capacity grew
-      SB_CUDA(c, cudaMalloc(&sl.pts, c->pts_cap * 16));
-      SB_CUDA(c, cudaMalloc(&sl.labels, c->pts_cap * 4));
-      SB_CUDA(c, cudaMalloc(&sl.probs, c->pts_cap * 4));
+      SB_CUDA(c, dev_alloc(sl.pts, c->pts_cap * 16));
+      SB_CUDA(c, dev_alloc(sl.labels, c->pts_cap * 4));
+      SB_CUDA(c, dev_alloc(sl.probs, c->pts_cap * 4));
     }
   sb_ctx::PrefetchSlot* slot = nullptr;
   for (auto& sl : c->prefetch)  // a slot that neither holds an unconsumed scan nor feeds the scan in flight
@@ -1806,10 +1729,10 @@ int sb_set_current_pose(sb_ctx* c, const double pose[16]) {  // SurfelMapping::s
   cudaSetDevice(c->device);
   memcpy(c->currentPose, pose, sizeof(c->currentPose));
   // the pose also lives on the device (PoseDev::currentPose): the next scan chains its increment onto it
-  SB_CUDA(c, cudaMemcpyAsync((char*)c->pd + offsetof(PoseDev, currentPose), c->currentPose, sizeof(c->currentPose),
-                             cudaMemcpyHostToDevice, c->stream));
+  SB_CUDA(c, cudaMemcpyAsync(c->res->pose.currentPose, c->currentPose, sizeof(c->currentPose), cudaMemcpyHostToDevice,
+                             c->stream));
   SB_CUDA(c, cudaStreamSynchronize(c->stream));
-  c->rkey_valid = false;
+  c->memo.clear();
   return SB_OK;
 }
 
@@ -1878,7 +1801,7 @@ int sb_comm_export(sb_ctx* c, uint8_t handle[64]) {
     // A CUDA IPC handle names the whole underlying allocation and cudaIpcOpenMemHandle returns ITS base: small
     // cudaMalloc requests are carved out of shared 2 MiB blocks, so an 8 KiB mailbox would be opened at the wrong
     // address on the peer. A 2 MiB allocation owns its block: exported pointer == base.
-    SB_CUDA(c, cudaMalloc(&c->mailbox, 2u << 20));
+    SB_CUDA(c, dev_alloc(c->mailbox, 2u << 20));
   }
   // Every export starts a fresh session: stamps of an earlier session must not match the epochs of the next one (both
   // restart at 1). Peers cannot write yet -- they only learn this mailbox's address from the handle returned here.
@@ -1917,7 +1840,7 @@ int sb_comm_init(sb_ctx* c, int rank, int nranks, const uint8_t* handles, int ro
   SB_CUDA(c, cudaMemset(c->comm_epoch, 0, 64));
   c->row_begin = row_begin;
   c->row_end = row_end;
-  c->comm_on = nranks > 1 || getenv("SUMA_B200_SELF_COMM") != nullptr;  // 1-rank loop-back: exercises the exchange on one GPU
+  c->comm_on = true;  // with nranks == 1 the exchange loops back to the own mailbox
   return SB_OK;
 }
 

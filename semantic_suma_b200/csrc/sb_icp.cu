@@ -166,40 +166,6 @@ __device__ __forceinline__ void icp_pixel(const KParams& kp, const IcpArgs& a, c
   icp_pixel_v(kp, a, M, pix, __ldg(a.data_v + pix), __ldg(a.data_n + pix), iteration, acc);
 }
 
-__device__ __forceinline__ long long warp_sum_ll(long long v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
-  return v;
-}
-
-// block-level reduction of Acc into 32 global int64 accumulators
-template <bool kFence>
-__device__ __forceinline__ void block_reduce_to_global(Acc& acc, long long* __restrict__ g_acc) {
-  __shared__ long long sm[kIcpThreads / 32][32];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-  for (int i = 0; i < 29; ++i) {
-    long long v = warp_sum_ll(acc.s[i]);
-    if (lane == 0) sm[warp][i] = v;
-  }
-  int nv = __reduce_add_sync(0xffffffffu, acc.n_valid);
-  int no = __reduce_add_sync(0xffffffffu, acc.n_outlier);
-  int ni = __reduce_add_sync(0xffffffffu, acc.n_invalid);
-  if (lane == 0) {
-    sm[warp][29] = nv;
-    sm[warp][30] = no;
-    sm[warp][31] = ni;
-  }
-  __syncthreads();
-  if (warp == 0) {
-    long long v = 0;
-#pragma unroll
-    for (int w = 0; w < kIcpThreads / 32; ++w) v += sm[w][lane];
-    if (v != 0) atomicAdd((unsigned long long*)(g_acc + lane), (unsigned long long)v);
-    if (kFence) __threadfence();
-  }
-}
-
 // Warp-level reduction of 32 values x 32 lanes with a transposing butterfly: at every step each lane keeps half of its
 // values and trades the other half with its partner, so the whole reduction costs 16+8+4+2+1 = 31 exchanges instead of
 // 32 x 5. Afterwards lane l holds the warp total of value l. (int64, so the association order is irrelevant.)
@@ -657,7 +623,7 @@ __global__ void __launch_bounds__(kIcpThreads, 2) k_gn_persistent(KParams kp, Gn
   // every iteration. Only when the whole stripe fits (<= kGnCachePix pixels per thread) and the objective is fixed.
   const int px_begin = job.a.row_begin * kp.W, px_end = job.a.row_end * kp.W;
   const int px_stride = gridDim.x * blockDim.x, px_first = px_begin + blockIdx.x * blockDim.x + threadIdx.x;
-  const bool cached = job.use_cache && job.mode != GN_POST && (px_end - px_begin) <= kGnCachePix * px_stride;
+  const bool cached = job.mode != GN_POST && (px_end - px_begin) <= kGnCachePix * px_stride;
   if (cached) {
 #pragma unroll
     for (int j = 0; j < kGnCachePix; ++j) {
@@ -903,7 +869,7 @@ int launch_gn_persistent(const Launch& L, const KParams& kp, const GnJob& job, l
     ScopedKernel sk(L, job.mode == GN_POST ? K_ICP_POST : K_ICP_FUSED);
     // the deeper cache only where the shallow one does not hold the stripe but the deep one does
     const long long px = (long long)(job.a.row_end - job.a.row_begin) * kp.W, per_pass = (long long)blocks * kIcpThreads;
-    const bool deep = job.use_cache && job.mode != GN_POST && px > 2 * per_pass && px <= 4 * per_pass;
+    const bool deep = job.mode != GN_POST && px > 2 * per_pass && px <= 4 * per_pass;
     e = cudaLaunchCooperativeKernel(deep ? (void*)k_gn_persistent<4> : (void*)k_gn_persistent<2>, dim3(blocks),
                                     dim3(kIcpThreads), args, 0, L.stream);
   }

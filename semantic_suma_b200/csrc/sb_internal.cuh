@@ -6,6 +6,8 @@
 #include <stdint.h>
 #include <string.h>
 
+#include <cstddef>
+#include <memory>
 #include <vector>
 
 #include "../../include/suma_b200.h"
@@ -58,7 +60,8 @@ struct SurfelPlanes {
 };
 
 // ---- device state of one fused Gauss-Newton run (LieGaussNewton.cpp:13-79) ----
-struct GnState {
+// GnHead is the part the host reads back after a run (and writes when it drives the loop itself)
+struct GnHead {
   double pose[16];       // Tk_
   double last_error;     // last_error
   double out48[48];      // sums of the last evaluated iteration
@@ -66,6 +69,8 @@ struct GnState {
   int done;              // loop left (converged or max iterations)
   int history_len;
   int error;             // a bounded spin of the persistent kernel timed out (missing block / peer GPU)
+};
+struct GnState : GnHead {
   double history[(kMaxGnIter + 1) * 16];
 };
 
@@ -74,10 +79,10 @@ struct IcpArgs {
   const float4* model_v; const float4* model_n; const float4* model_s;
   float distance_thresh, angle_thresh;  // Frame2Model.cpp:66-67
   int row_begin, row_end;
-  int has_semantics;
-  int row_step;  // row permutation stride of the work distribution, coprime to (row_end - row_begin)
   int Wm, Hm;    // size of the model images = textureSize(vertex_model) (Frame2Model_jacobians.geom:70): the rendered
                  // model frame, or the last data frame in the frame-to-frame fallback (SurfelMapping.cpp:442)
+  // (this order leaves k_gn_persistent<2> with 24 bytes of spill loads; with has_semantics ahead of Wm it takes 68)
+  int has_semantics;
 };
 
 // peer mailboxes for the multi-GPU one-shot all-reduce (fused into the Jacobian kernel's last block)
@@ -107,6 +112,43 @@ struct PoseDev {
   float t_err, r_err;
   int pad2[2];
 };
+
+// The per-scan results in one device block, so that the end of a scan is a single device-to-host copy into its pinned
+// mirror. The offsets are those of the original hand-laid block; the copy moves all 8256 bytes.
+struct ResultBlock {
+  PoseDev pose;                       // device-resident pose bookkeeping of the pipeline
+  char pad0[4096 - sizeof(PoseDev)];
+  long long sums[64];                 // raw sums of a Jacobian pass (the first 32; the scan's statistics pass)
+  char pad1[8192 - 4096 - 64 * sizeof(long long)];
+  uint32_t counts[16];  // [0] n surfels, [1] n after update (base for new), [2] kept updated, [3] kept new, [4] extracted
+};
+static_assert(offsetof(ResultBlock, sums) == 4096, "result block layout");
+static_assert(offsetof(ResultBlock, counts) == 8192, "result block layout");
+static_assert(sizeof(ResultBlock) == 8256, "result block layout");
+
+// Owning handle of one allocation. It converts to the plain pointer that launchers and sub-views take.
+template <class T, class Free>
+struct Owned : std::unique_ptr<T, Free> {
+  using std::unique_ptr<T, Free>::unique_ptr;
+  operator T*() const { return this->get(); }
+};
+struct CudaFree {
+  void operator()(void* p) const { cudaFree(p); }
+};
+struct CudaFreeHost {
+  void operator()(void* p) const { cudaFreeHost(p); }
+};
+template <class T>
+using DevPtr = Owned<T, CudaFree>;
+template <class T>
+using PinnedPtr = Owned<T, CudaFreeHost>;
+template <class T>
+cudaError_t dev_alloc(DevPtr<T>& p, size_t bytes) {
+  void* raw = nullptr;
+  cudaError_t e = cudaMalloc(&raw, bytes);
+  p.reset(static_cast<T*>(raw));
+  return e;
+}
 
 // ---------------- kernel ids (launch accounting + the optional CUDA-event profiler) ----------------
 enum KernelId {
@@ -155,9 +197,8 @@ struct ScopedKernel {
 // sb_preprocess.cu
 // the two alternating z-buffer key images of the scan projection ([H][W+6] each, see sb_preprocess.cu) and their TMA maps
 struct PrepKeys {
-  unsigned long long* img[2] = {nullptr, nullptr};
+  DevPtr<unsigned long long> img[2];
   int cur = 0;
-  bool use_tma = false;
   bool tmap_ok[2] = {false, false};
   CUtensorMap tmap[2];
 };
@@ -187,7 +228,6 @@ struct GnJob {
   int max_iter;
   double eps, delta;
   unsigned int epoch_base;
-  int use_cache;  // keep the thread's data pixels in shared memory across iterations
 };
 void launch_gn_init(const Launch& L, GnState* st, const Mat4d& T0, long long* acc32);
 int launch_gn_persistent(const Launch& L, const KParams& kp, const GnJob& job, long long* slots, unsigned int* ticket,

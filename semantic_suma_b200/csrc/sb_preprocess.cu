@@ -289,7 +289,7 @@ void launch_preprocess(const Launch& L, const KParams& kp, const float4* pts, co
   dim3 grid((kp.W + kPrepTX - 1) / kPrepTX, (kp.H + kPrepTY - 1) / kPrepTY);
   {
     ScopedKernel sk(L, K_PREPROCESS_TILE);
-    if (keys.use_tma && keys.tmap_ok[keys.cur])
+    if (keys.tmap_ok[keys.cur])
       k_preprocess_tile<true><<<grid, kPrepThreads, 0, L.stream>>>(kp, io, keys.tmap[keys.cur]);
     else
       k_preprocess_tile<false><<<grid, kPrepThreads, 0, L.stream>>>(kp, io, keys.tmap[keys.cur]);

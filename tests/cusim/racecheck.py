@@ -30,7 +30,6 @@ def child(n_scans, width):
     product_build.LIB = path
     product_build.build = lambda *a, **k: path
     from semantic_suma_b200 import api, synth
-    os.environ["SUMA_B200_SELF_COMM"] = "1"
     pp = api.default_params(data_width=width, model_width=width, max_iterations=4, stopping_threshold=0.0, delta=0.0)
     sl = api.SurfelMapping(pp)
     h = np.zeros(64, np.uint8)

@@ -176,6 +176,55 @@ def test_map_update_and_render_bit_exact_semantic():
     _run_map_sequence(900, 5, True)
 
 
+def _map_for_render(po, ctx, n=3):
+    """a small map built from seeded scans, and a pose to render it at"""
+    sc, poses = scans(900, n=n)
+    gmap = api.SurfelMap(ctx)
+    for t in range(n):
+        _, f = _prep_both(po, ctx, sc[t], t)
+        gmap.update((np.linalg.inv(poses[0]) @ poses[t]).astype(np.float32), f)
+    return gmap, sc, (np.linalg.inv(poses[0]) @ poses[n - 1]).astype(np.float32)
+
+
+def test_render_after_preprocess_into_the_render_target():
+    """the render memo must not outlive a preprocessing pass that overwrote the frame it rendered into (data size ==
+    model size, so one frame can be both)"""
+    po, pp = both_params(**sized(900))
+    ctx = api.Context(pp)
+    gmap, sc, pose = _map_for_render(po, ctx)
+    F = api.Frame(ctx, 900, 64)
+    gmap.render(pose, pose, F, 0.0)
+    pts, lab, prb = sc[0]
+    api.Preprocessing(ctx).process(pts, F, lab, prb, 0)
+    gmap.render(pose, pose, F, 0.0)
+    fresh = api.Frame(ctx, 900, 64)
+    gmap.render(pose, pose, fresh, 0.0)
+    for g, o, name in zip(F.maps(), fresh.maps(), ("vertex", "normal", "semantic")):
+        assert_bits_equal(g, o, "render after preprocess %s" % name)
+    assert (fresh.vertex_map[..., 3] > 0).sum() > 1000
+    ctx.close()
+
+
+def test_render_into_a_frame_created_after_destroying_the_last_target():
+    """the render memo must not take a new frame for the destroyed one it rendered into, at the same address or not"""
+    po, pp = both_params(**sized(900))
+    ctx = api.Context(pp)
+    gmap, _, pose = _map_for_render(po, ctx)
+    F = api.Frame(ctx, 900, 64)
+    gmap.render(pose, pose, F, 0.0)
+    want = F.maps()
+    addr = F.h.value
+    api.lib().sb_frame_destroy(F.h)
+    F.h = None
+    G = api.Frame(ctx, 900, 64)
+    same_address = G.h.value == addr
+    print("re-created frame at the destroyed frame's address: %s" % same_address)
+    gmap.render(pose, pose, G, 0.0)
+    for g, o, name in zip(G.maps(), want, ("vertex", "normal", "semantic")):
+        assert_bits_equal(g, o, "render into a re-created frame (same handle: %s) %s" % (same_address, name))
+    ctx.close()
+
+
 def test_map_render_old_surfels():
     # surfels older than the compose age (100 scans) exercise the old / composed views
     po, pp = both_params(**sized(900))
@@ -372,7 +421,6 @@ def test_fused_peer_exchange_in_one_gpu_loop_back():
     """the in-kernel all-reduce of the striped Gauss-Newton loop (store sums + epoch stamp into every rank's mailbox,
     spin on the own mailbox) executed with nranks = 1 -- the driver's single-GPU box runs the exchange code path"""
     import ctypes as C
-    import os
     po, pp = both_params(**sized(900, max_iterations=8, stopping_threshold=0.0, delta=0.0))
     sc, _ = scans(900, n=4)
     solo = api.SurfelMapping(pp)
@@ -380,20 +428,16 @@ def test_fused_peer_exchange_in_one_gpu_loop_back():
         solo.processScan(*s)
     ref_pose, ref_n = solo.getCurrentPose().copy(), solo.getMap().size()
     solo.ctx.close()
-    os.environ["SUMA_B200_SELF_COMM"] = "1"
-    try:
-        sl = api.SurfelMapping(pp)
-        h = np.zeros(64, np.uint8)
-        L = api.lib()
-        sl.ctx.check(L.sb_comm_export(sl.ctx.h, C.c_void_p(h.ctypes.data)), "export")
-        sl.ctx.check(L.sb_comm_init(sl.ctx.h, 0, 1, C.c_void_p(h.ctypes.data), 0, pp.data_height), "init")
-        for s in sc:
-            sl.processScan(*s)
-        assert_bits_equal(sl.getCurrentPose(), ref_pose, "pose with the exchange in the loop")
-        assert sl.getMap().size() == ref_n
-        sl.ctx.close()
-    finally:
-        del os.environ["SUMA_B200_SELF_COMM"]
+    sl = api.SurfelMapping(pp)
+    h = np.zeros(64, np.uint8)
+    L = api.lib()
+    sl.ctx.check(L.sb_comm_export(sl.ctx.h, C.c_void_p(h.ctypes.data)), "export")
+    sl.ctx.check(L.sb_comm_init(sl.ctx.h, 0, 1, C.c_void_p(h.ctypes.data), 0, pp.data_height), "init")
+    for s in sc:
+        sl.processScan(*s)
+    assert_bits_equal(sl.getCurrentPose(), ref_pose, "pose with the exchange in the loop")
+    assert sl.getMap().size() == ref_n
+    sl.ctx.close()
 
 
 def test_cuda_equals_reference_shaders_directly():
