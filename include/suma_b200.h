@@ -88,6 +88,13 @@ enum { SB_SLAM_CURRENT = 0, SB_SLAM_LAST = 1, SB_SLAM_CURRENT_MODEL = 2, SB_SLAM
 
 /* ---- context ---------------------------------------------------------------------------------------------- */
 int sb_default_params(sb_params* p);                               /* config/default.xml */
+/* sb_create and sb_set_params return SB_ERR_INVALID (reason on stderr / in sb_last_error) for:
+ *  - image sizes <= 0, more than 2^24 data pixels, or a data width of 1 (the preprocessing stencils reach two columns
+ *    around the azimuth seam, which one column cannot provide);
+ *  - depth ranges with max <= min;
+ *  - parameters whose exact ICP sums could leave the int64 range: data pixels x (max(max_depth, model_max_depth) + 25 m)^2
+ *    x 2^30 > 2^63 - 1. The 25 m allow for the translation of the pose. 128x4096 at 75 m is accepted; the largest image
+ *    at 75 m has 858 993 pixels. */
 int sb_create(const sb_params* p, int device, sb_ctx** out);       /* SurfelMapping::SurfelMapping, SurfelMapping.cpp:19 */
 int sb_destroy(sb_ctx* ctx);
 int sb_reset(sb_ctx* ctx);                                         /* SurfelMapping::reset / SurfelMap::reset, SurfelMap.cpp:473 */

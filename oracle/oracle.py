@@ -73,6 +73,7 @@ def lib():
         for n in ("asinf", "acosf", "sinf", "expf", "logf"):
             f = getattr(L, "orc_t_" + n); f.restype = C.c_float; f.argtypes = [C.c_float]
         L.orc_t_sincos.argtypes = [C.c_double, C.POINTER(C.c_double), C.POINTER(C.c_double)]
+        L.orc_check_params.restype = C.c_char_p
         L.orc_map_create.restype = C.c_void_p
         L.orc_slam_create.restype = C.c_void_p
         L.orc_slam_map.restype = C.c_void_p
@@ -118,6 +119,19 @@ def default_params(**kw):
             raise KeyError(k)
         setattr(p, k, v)
     return p
+
+
+def check_params(p):
+    """None if sb_create accepts these parameters, otherwise the reason it refuses them (orc_check_params)"""
+    why = lib().orc_check_params(C.byref(p))
+    return None if why is None else why.decode()
+
+
+def _create(fn, p):
+    why = check_params(p)
+    if why is not None:
+        raise ValueError("parameters refused: " + why)
+    return C.c_void_p(fn(C.byref(p)))
 
 
 def colmajor(T, dtype):
@@ -220,7 +234,8 @@ class Map:
     def __init__(self, p, handle=None):
         self.p = p
         self._own = handle is None
-        self.h = C.c_void_p(lib().orc_map_create(C.byref(p))) if handle is None else C.c_void_p(handle)
+        self.h = None
+        self.h = _create(lib().orc_map_create, p) if handle is None else C.c_void_p(handle)
 
     def __del__(self):
         if getattr(self, "_own", False) and self.h:
@@ -292,7 +307,8 @@ class Map:
 class Slam:
     def __init__(self, p):
         self.p = p
-        self.h = C.c_void_p(lib().orc_slam_create(C.byref(p)))
+        self.h = None
+        self.h = _create(lib().orc_slam_create, p)
         self.map = Map(p, handle=lib().orc_slam_map(self.h))
         self.loop = None
 

@@ -83,6 +83,9 @@ typedef struct orc_surfel {
 } orc_surfel;
 
 void orc_default_params(orc_params* p); /* config/default.xml */
+/* the parameters the CUDA library's sb_create accepts: NULL, or the reason they are refused. orc_map_create and
+ * orc_slam_create return NULL on refused parameters. */
+const char* orc_check_params(const orc_params* p);
 /* host threads used by the oracle's loops (OpenMP); 0 = all the machine offers (capped at 64). Results are
  * bit-identical for every thread count. Returns the count now in effect. */
 int orc_set_threads(int n);

@@ -54,6 +54,19 @@ void orc_default_params(orc_params* p) {
   p->label_offset_quirk = 1; p->render_after_update = 1;
 }
 
+/* the rule of sb_create: image sizes, and the Q33.30 head-room of the exact ICP sums -- data pixels x (the longer of the
+ * two depth ranges + 25 m for the pose's translation)^2 x 2^30 must stay within int64 (DESIGN.md section 2) */
+const char* orc_check_params(const orc_params* p) {
+  if (p->data_width <= 0 || p->data_height <= 0 || p->model_width <= 0 || p->model_height <= 0) return "image size <= 0";
+  if ((size_t)p->data_width * p->data_height > (1u << 24)) return "more than 2^24 data pixels";
+  if (p->data_width < 2) return "data width < 2";
+  if (!(p->max_depth > p->min_depth) || !(p->model_max_depth > p->model_min_depth)) return "max depth <= min depth";
+  const double range = (p->max_depth > p->model_max_depth ? p->max_depth : p->model_max_depth) + 25.0;
+  if ((double)p->data_width * p->data_height * range * range * 1073741824.0 > 9223372036854775807.0)
+    return "data pixels x (max depth + 25 m)^2 x 2^30 exceeds the int64 range of the exact ICP sums";
+  return NULL;
+}
+
 float orc_t_atan2f(float y, float x) { return orc_atan2f(y, x); }
 float orc_t_asinf(float x) { return orc_asinf(x); }
 float orc_t_acosf(float x) { return orc_acosf(x); }

@@ -84,6 +84,7 @@ static void orc_map_derive(orc_map* m) {
 }
 
 orc_map* orc_map_create(const orc_params* p) {
+  if (orc_check_params(p)) return NULL;
   orc_map* m = (orc_map*)calloc(1, sizeof(orc_map));
   m->p = *p;
   size_t Pm = (size_t)p->model_width * p->model_height, Pd = (size_t)p->data_width * p->data_height;

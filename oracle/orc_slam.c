@@ -34,6 +34,7 @@ static void cast_f(const double* M, float* F) { for (int i = 0; i < 16; ++i) F[i
 static double now_s(void) { struct timespec ts; clock_gettime(CLOCK_MONOTONIC, &ts); return ts.tv_sec + 1e-9 * ts.tv_nsec; }
 
 orc_slam* orc_slam_create(const orc_params* p) {
+  if (orc_check_params(p)) return NULL;
   orc_slam* s = (orc_slam*)calloc(1, sizeof(orc_slam));
   s->p = *p;
   s->map = orc_map_create(p);

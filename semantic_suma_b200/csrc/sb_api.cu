@@ -1137,16 +1137,33 @@ int sb_device_count(void) {
   return n;
 }
 
-static int check_params(const sb_params* p) {
-  if (!p) return SB_ERR_INVALID;
-  if (p->data_width <= 0 || p->data_height <= 0 || p->model_width <= 0 || p->model_height <= 0) return SB_ERR_INVALID;
-  if ((size_t)p->data_width * p->data_height > (1u << 24)) return SB_ERR_INVALID;
-  if (!(p->max_depth > p->min_depth) || !(p->model_max_depth > p->model_min_depth)) return SB_ERR_INVALID;
-  return SB_OK;
+// Head-room of the exact ICP sums. The largest per-pixel term is |v_d x n_m|^2 <= |v_d|^2 (unit normals), or r^2 for F,
+// with the residual r at most about the longer range of a data / model pair on one beam. |v_d| is the data range plus
+// the translation of the pose the data is moved by: kIcpPoseMargin metres of it are allowed for. At 75 m, 128x4096
+// (5.6e18 of 9.2e18) is accepted; the largest image accepted at 75 m has 858 993 pixels.
+constexpr double kIcpPoseMargin = 25.0;
+
+// Parameters the library cannot run with exactly: nullptr when fine, otherwise the reason.
+static const char* check_params(const sb_params* p) {
+  if (!p) return "no parameters";
+  if (p->data_width <= 0 || p->data_height <= 0 || p->model_width <= 0 || p->model_height <= 0) return "image size <= 0";
+  if ((size_t)p->data_width * p->data_height > (1u << 24)) return "more than 2^24 data pixels";
+  // the stencils of preprocessing reach 2 columns around the azimuth seam; one column cannot wrap onto itself twice
+  if (p->data_width < 2) return "data width < 2";
+  if (!(p->max_depth > p->min_depth) || !(p->model_max_depth > p->model_min_depth)) return "max depth <= min depth";
+  // Q33.30 head-room of the exact ICP sums: no int64 sum may wrap (DESIGN.md section 2)
+  const double range = (p->max_depth > p->model_max_depth ? p->max_depth : p->model_max_depth) + kIcpPoseMargin;
+  if ((double)p->data_width * p->data_height * range * range * 1073741824.0 > 9223372036854775807.0)
+    return "data pixels x (max depth + 25 m)^2 x 2^30 exceeds the int64 range of the exact ICP sums";
+  return nullptr;
 }
 
 int sb_create(const sb_params* p, int device, sb_ctx** out) {
-  if (!out || check_params(p)) return SB_ERR_INVALID;
+  if (!out) return SB_ERR_INVALID;
+  if (const char* why = check_params(p)) {
+    fprintf(stderr, "sb_create: %s\n", why);
+    return SB_ERR_INVALID;
+  }
   int n = 0;
   if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) return SB_ERR_NOGPU;  // no CPU fallback
   if (device < 0 || device >= n) return SB_ERR_INVALID;
@@ -1216,7 +1233,8 @@ int sb_reset(sb_ctx* c) {
 }
 
 int sb_set_params(sb_ctx* c, const sb_params* p) {
-  if (!c || check_params(p)) return fail(c, SB_ERR_INVALID, "set_params: bad parameters");
+  if (!c) return SB_ERR_INVALID;
+  if (const char* why = check_params(p)) return fail(c, SB_ERR_INVALID, std::string("set_params: ") + why);
   if (p->data_width != c->p.data_width || p->data_height != c->p.data_height || p->model_width != c->p.model_width ||
       p->model_height != c->p.model_height)
     return fail(c, SB_ERR_STATE, "set_params: image sizes are fixed at sb_create (as in SurfelMapping's constructor)");

@@ -758,7 +758,8 @@ __global__ void __launch_bounds__(kThreads) k_radius(KParams kp, FrameDev f, flo
   if (pix >= kp.W * kp.H) return;
   index_keys[pix] = ~0ull;
   integrated[pix] = 0;
-  if (pix < kGroupCounts) group_counts[pix] = 0;
+  // all kGroupCounts totals, also on an image of fewer pixels: the compaction reads every group the map spans
+  for (int g = pix; g < kGroupCounts; g += kp.W * kp.H) group_counts[g] = 0;
   float4 V = __ldg(f.vertex + pix), N = __ldg(f.normal + pix);
   float4 o = make_float4(0.f, 0.f, 0.f, 0.f);
   V3 v = mk3(V.x, V.y, V.z), n = mk3(N.x, N.y, N.z);

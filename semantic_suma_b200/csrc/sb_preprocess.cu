@@ -238,7 +238,8 @@ __global__ void __launch_bounds__(kPrepThreads) k_preprocess_tile(KParams kp, Pr
     }
     if (io.index_keys) io.index_keys[pix] = ~0ull;
     if (io.integrated) io.integrated[pix] = 0;
-    if (io.group_counts && pix < (size_t)kGroupCounts) io.group_counts[pix] = 0;
+    if (io.group_counts)  // all of them, also on an image of fewer pixels (see k_radius)
+      for (size_t g = pix; g < (size_t)kGroupCounts; g += (size_t)W * H) io.group_counts[g] = 0;
     // re-arm the other key image (own pixel and its mirror copies in the pads)
     unsigned long long* row = io.keys_next + (size_t)gy * Wp;
     row[gx + kPrepHalo] = ~0ull;

@@ -49,6 +49,12 @@ def test_cuda_sources_on_the_cpu_executor_equal_the_oracle():
     assert n >= 28
 
 
+def test_map_update_on_an_image_under_256_pixels():
+    """three updates of a 3.6 M-surfel map with a 16x8 frame: all 256 group totals of the update pass are cleared, not only
+    the first P (tests/test_gpu_shapes.py)"""
+    assert _child(["tests/test_gpu_shapes.py"], "test_map_updates_on_an_image_under_256_pixels") == 1
+
+
 @long_run
 def test_kernel_results_do_not_depend_on_the_execution_order():
     """CUDA promises no order between the lanes of a warp or the warps of a block outside its synchronisation primitives:
