@@ -2,6 +2,7 @@
 // (Preprocessing::process, SurfelMap::render*/update, Frame2Model::jacobianProducts, LieGaussNewton::minimize) and the
 // per-scan orchestration of SurfelMapping::processScan (core/SurfelMapping.cpp:175-210, 323-358, 372-476, 797-804).
 // There is no CPU fallback: without a CUDA device sb_create fails with SB_ERR_NOGPU.
+#include <algorithm>
 #include <chrono>
 #include <cmath>
 #include <cstddef>
@@ -93,7 +94,6 @@ struct sb_ctx {
   DevPtr<float4> A_mem, T_mem, G_mem, X_mem;
   DevPtr<uint8_t> keep;
   DevPtr<uint32_t> block_counts;
-  DevPtr<uint32_t> block_offsets;
   DevPtr<unsigned long long> lb_desc;  // look-back descriptors of the single-pass compactions
   DevPtr<uint32_t> lb_ticket;
   uint32_t lb_gen = 0;
@@ -109,7 +109,7 @@ struct sb_ctx {
   DevPtr<unsigned long long> key_index;
   DevPtr<float4> radius_map;
   DevPtr<uint8_t> integrated;
-  DevPtr<uint32_t> group_counts;  // kGroupCounts totals of the update pass (64 blocks each)
+  DevPtr<uint32_t> group_counts;  // kGroupCounts totals of the update pass / a tile extraction (64 blocks each)
   FramePtr f_old, f_new, f_comp;
   uint64_t frames_created = 0;
   uint32_t n_host = 0;   // surfel count (exact; refreshed after every update)
@@ -121,8 +121,7 @@ struct sb_ctx {
   std::map<std::pair<int32_t, int32_t>, DevTile> tiles;
   SurfelPlanes pool{};            // tile cache lanes
   DevPtr<float4> pool_mem;
-  DevPtr<uint32_t> d_pool_top;
-  DevPtr<uint2> d_tile_rec;       // {base, count} per extraction
+  DevPtr<uint2> d_tile_rec;       // {end in the pool, surfels of the tile} per extraction; slot s starts at the end of s - 1
   uint32_t n_slots = 0;
   bool tiles_pending = false;     // some records have not been read back yet
 
@@ -278,7 +277,6 @@ int reset_state(sb_ctx* c) {
   c->stats[12] = 0.0;
   c->loop.reset();  // posegraph_->clear(); trajectory_distances_ ... (SurfelMapping.cpp:158-163)
   for (int i = 0; i < 16; ++i) c->lastPose_old[i] = (i % 5 == 0) ? 1.0 : 0.0;
-  SB_CUDA(c, cudaMemsetAsync(c->d_pool_top, 0, 64, c->stream));
   c->h_poses.assign((size_t)kMaxPoses * 16, 0.0f);
   for (uint32_t t = 0; t < kMaxPoses; ++t)
     for (int i = 0; i < 4; ++i) c->h_poses[16 * (size_t)t + 5 * i] = 1.0f;
@@ -345,12 +343,10 @@ int alloc_buffers(sb_ctx* c) {
   if ((r = alloc_planes(c, c->G_mem, &c->G, Pd))) return r;
   if ((r = alloc_planes(c, c->X_mem, &c->X, 16))) return r;
   if ((r = alloc_planes(c, c->pool_mem, &c->pool, kTilePoolCap))) return r;
-  SB_CUDA(c, dev_alloc(c->d_pool_top, 64));
   SB_CUDA(c, dev_alloc(c->d_tile_rec, (size_t)kMaxTileSlots * sizeof(uint2)));
   SB_CUDA(c, dev_alloc(c->keep, kMaxSurfels));
   size_t nb = (kMaxSurfels + 127) / 128 + 16;  // blocks of the finest-grained surfel kernel
   SB_CUDA(c, dev_alloc(c->block_counts, nb * 4));
-  SB_CUDA(c, dev_alloc(c->block_offsets, nb * 4));
   SB_CUDA(c, dev_alloc(c->lb_desc, (nb + 16) * 8));
   SB_CUDA(c, cudaMemsetAsync(c->lb_desc, 0, (nb + 16) * 8, c->stream));
   SB_CUDA(c, dev_alloc(c->lb_ticket, 64));
@@ -653,25 +649,27 @@ int fetch_counts(sb_ctx* c, uint32_t* dst, int n) {
   return SB_OK;
 }
 
-int refresh_tile_records(sb_ctx* c) {  // read back {base, count} of the tiles extracted so far
+int refresh_tile_records(sb_ctx* c) {  // read back the records of the tiles extracted so far
   if (!c->tiles_pending || c->n_slots == 0) return SB_OK;
   std::vector<uint2> rec(c->n_slots);
   SB_CUDA(c, cudaMemcpyAsync(rec.data(), c->d_tile_rec, (size_t)c->n_slots * sizeof(uint2), cudaMemcpyDeviceToHost,
                              c->stream));
   SB_CUDA(c, cudaStreamSynchronize(c->stream));
-  {  // surfels that did not fit the 16 M-surfel HBM tile pool (the reference's host-side cache is unbounded)
-    uint32_t top[2] = {0, 0};
-    SB_CUDA(c, cudaMemcpy(top, c->d_pool_top, sizeof(top), cudaMemcpyDeviceToHost));
-    if (top[1] != (uint32_t)c->stats[12]) {
-      c->stats[12] = top[1];
-      c->err = "submap tile pool exhausted: " + std::to_string(top[1]) + " surfels of leaving tiles were dropped";
+  auto base = [&](uint32_t s) { return s ? rec[s - 1].x : 0u; };
+  {  // surfels that did not fit the 16 M-surfel HBM tile pool (the reference's host-side cache is unbounded); slots are
+     // never reused, so the sum over all slots counts every drop since the last reset
+    uint64_t dropped = 0;
+    for (uint32_t s = 0; s < c->n_slots; ++s) dropped += std::min(rec[s].y, kExtractCap) - (rec[s].x - base(s));
+    if ((double)dropped != c->stats[12]) {
+      c->stats[12] = (double)dropped;
+      c->err = "submap tile pool exhausted: " + std::to_string(dropped) + " surfels of leaving tiles were dropped";
     }
   }
   for (auto& kv : c->tiles) {
     DevTile& t = kv.second;
     if (!t.known) {
-      t.base = rec[t.slot].x;
-      t.count = rec[t.slot].y;
+      t.base = base(t.slot);
+      t.count = rec[t.slot].x - t.base;
       t.known = true;
     }
   }
@@ -691,10 +689,10 @@ int append_tiles(sb_ctx* c, int32_t i0, int32_t j0, int di, int dj) {  // Surfel
     uint32_t room = kMaxSurfels - c->n_host;
     uint32_t n = t.count < room ? t.count : room;
     if (n == 0) continue;
-    SB_CUDA(c, cudaMemcpyAsync(c->A.p0 + c->n_host, c->pool.p0 + t.base, (size_t)n * 16, cudaMemcpyDeviceToDevice, c->stream));
-    SB_CUDA(c, cudaMemcpyAsync(c->A.p1 + c->n_host, c->pool.p1 + t.base, (size_t)n * 16, cudaMemcpyDeviceToDevice, c->stream));
-    SB_CUDA(c, cudaMemcpyAsync(c->A.p2 + c->n_host, c->pool.p2 + t.base, (size_t)n * 16, cudaMemcpyDeviceToDevice, c->stream));
-    SB_CUDA(c, cudaMemcpyAsync(c->A.p3 + c->n_host, c->pool.p3 + t.base, (size_t)n * 16, cudaMemcpyDeviceToDevice, c->stream));
+    // the four lanes of A and of the pool lie at fixed pitches (kMaxSurfels, kTilePoolCap) in one allocation each
+    for (size_t lane = 0; lane < 4; ++lane)
+      SB_CUDA(c, cudaMemcpyAsync(c->A.p0 + lane * kMaxSurfels + c->n_host, c->pool.p0 + lane * kTilePoolCap + t.base,
+                                 (size_t)n * 16, cudaMemcpyDeviceToDevice, c->stream));
     c->n_host += n;
     c->n_upper = c->n_host;
     appended = true;
@@ -716,8 +714,10 @@ int extract_surfels(sb_ctx* c, bool partially) {
     if (c->n_slots >= kMaxTileSlots) return fail(c, SB_ERR_CAPACITY, "tile cache: out of record slots");
     float2 ctr = submap_center(c, idx.first, idx.second);
     uint32_t slot = c->n_slots++;
+    // extractions can follow each other with no per-pixel prologue in between to clear the group totals
+    SB_CUDA(c, cudaMemsetAsync(c->group_counts, 0, kGroupCounts * 4, c->stream));
     launch_extract_to_pool(L, c->A, c->res->counts, c->n_host, c->poses, ctr, c->p.submap_extent, c->keep, c->block_counts,
-                           c->block_offsets, c->pool, kTilePoolCap, c->d_pool_top, c->d_tile_rec + slot, kExtractCap);
+                           c->group_counts, c->pool, kTilePoolCap, c->d_tile_rec, slot, kExtractCap);
     DevTile t;
     t.slot = slot;
     t.known = false;
@@ -790,8 +790,8 @@ int map_update(sb_ctx* c, const float* pose, const sb_frame* frame, const Mat4* 
   launch_update_surfels(L, kp, c->A, c->T, c->res->counts, n_grid(c), mat4_from(pose_h), mat4_from(inv_pose), pose_dev,
                         inv_dev, c->poses, c->poses_inv, c->key_index, c->radius_map, frame->d, (int)c->map_timestamp,
                         ctr, extent, c->integrated, c->keep, c->block_counts, c->group_counts);
-  launch_compact_update(L, c->T, c->keep, c->block_counts, c->group_counts, c->res->counts, n_grid(c), c->A, kMaxSurfels,
-                        c->res->counts + 1, c->res->counts + 2);
+  launch_compact(L, c->T, c->keep, c->block_counts, c->group_counts, c->res->counts, n_grid(c), c->A, nullptr, kMaxSurfels,
+                 kMaxSurfels, c->res->counts + 1);
   // K6d + K6e: new surfels appended behind the updated ones; counts[0] = new map size, counts[3] = new surfels
   c->lb_gen = (c->lb_gen + 1) & 0x3fffffffu;
   if (c->lb_gen == 0) c->lb_gen = 1;

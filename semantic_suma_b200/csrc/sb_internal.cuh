@@ -22,7 +22,7 @@ constexpr uint32_t kComposeAge = 100u;           // SurfelMap.h:144
 constexpr int kMaxGnIter = 256;
 constexpr uint32_t kTilePoolCap = 16u * 1024u * 1024u;  // surfels held by the HBM tile cache (1 GiB)
 constexpr uint32_t kMaxTileSlots = 16384u;
-constexpr int kGroupCounts = 256;  // group totals of the update pass: kMaxSurfels / 256 threads / 64 blocks per group = 256
+constexpr int kGroupCounts = 256;  // group totals of a surfel-indexed compaction: kMaxSurfels / 256 threads / 64 blocks per group
 
 // everything the kernels need from sb_params plus the derived constants the reference computes on the host
 struct KParams {
@@ -154,7 +154,7 @@ cudaError_t dev_alloc(DevPtr<T>& p, size_t bytes) {
 enum KernelId {
   K_FILL = 0, K_PROJECT_SCATTER, K_PREPROCESS_TILE, K_ICP_JACOBIAN, K_GN_INIT,
   K_ICP_FUSED, K_POSE_PRODUCTS, K_RENDER_SCATTER, K_RENDER_RESOLVE, K_INDEX_SCATTER, K_RADIUS, K_UPDATE_SURFELS,
-  K_GEN_SURFELS, K_EXTRACT_FLAGS, K_SCAN_BLOCKS, K_COMPACT_SCATTER, K_AOS_TO_SOA, K_SOA_TO_AOS, K_ICP_POST, K_COUNT
+  K_GEN_SURFELS, K_EXTRACT_FLAGS, K_COMPACT_SCATTER, K_AOS_TO_SOA, K_SOA_TO_AOS, K_ICP_POST, K_COUNT
 };
 const char* kernel_name(int id);
 
@@ -259,9 +259,11 @@ void launch_index_scatter(const Launch& L, const KParams& kp, SurfelPlanes s, co
                           const float* M, unsigned long long* keys);
 void launch_radius(const Launch& L, const KParams& kp, FrameDev frame, float4* radius_map, unsigned long long* index_keys,
                    uint8_t* integrated, uint32_t* group_counts);
-void launch_compact_update(const Launch& L, SurfelPlanes src, const uint8_t* keep, const uint32_t* block_counts,
-                           const uint32_t* group_counts, const uint32_t* n_dev, uint32_t n_upper, SurfelPlanes dst,
-                           uint32_t cap, uint32_t* count_out, uint32_t* kept_out);
+// ordered compaction of a surfel-indexed pass: items flagged in keep[0..n) of src go to dst[base..) in order, base =
+// *base_dev (0 if null); out[0] = end of the written range, out[1] = number of items kept
+void launch_compact(const Launch& L, SurfelPlanes src, const uint8_t* keep, const uint32_t* block_counts,
+                    const uint32_t* group_counts, const uint32_t* n_dev, uint32_t n_upper, SurfelPlanes dst,
+                    const uint32_t* base_dev, uint32_t cap, uint32_t rel_cap, uint32_t* out);
 void launch_update_surfels(const Launch& L, const KParams& kp, SurfelPlanes src, SurfelPlanes tmp, const uint32_t* n_dev,
                            uint32_t n_upper, const Mat4& pose, const Mat4& inv_pose, const Mat4* pose_dev,
                            const Mat4* inv_pose_dev, const float* poses,
@@ -273,12 +275,11 @@ void launch_gen_compact(const Launch& L, const KParams& kp, FrameDev frame, cons
                         const uint8_t* integrated, const float* poses, int timestamp, float2 submap_center,
                         float submap_extent, SurfelPlanes map, unsigned long long* desc, uint32_t* ticket, uint32_t gen,
                         uint32_t cap, uint32_t* counts);
-// ordered compaction: items flagged in keep[0..n) of src go to dst[base..) in order; *count_out = base + #kept
+// the surfels of one submap tile, in order, into pool slot `slot`: rec[slot] = {end of the slot in the pool, surfels of
+// the tile}; slot s starts at the end of slot s - 1. The group totals must be zero.
 void launch_extract_to_pool(const Launch& L, SurfelPlanes map, const uint32_t* n_dev, uint32_t n_upper, const float* poses,
-                            float2 center, float extent, uint8_t* keep, uint32_t* block_counts, uint32_t* block_offsets,
-                            SurfelPlanes pool, uint32_t pool_cap, uint32_t* pool_top, uint2* rec, uint32_t tile_cap);
-void launch_extract_flags(const Launch& L, SurfelPlanes s, const uint32_t* n_dev, uint32_t n_upper, const float* poses,
-                          float2 center, float extent, uint8_t* keep, uint32_t* block_counts);
+                            float2 center, float extent, uint8_t* keep, uint32_t* block_counts, uint32_t* group_counts,
+                            SurfelPlanes pool, uint32_t pool_cap, uint2* rec, uint32_t slot, uint32_t tile_cap);
 void launch_aos_to_soa(const Launch& L, const sb_surfel* aos, SurfelPlanes s, uint32_t offset, uint32_t n);
 void launch_soa_to_aos(const Launch& L, SurfelPlanes s, sb_surfel* aos, uint32_t n);
 

@@ -9,8 +9,10 @@
 //    (depth24 << 40 | pass << 32 | surfel index): "earliest primitive wins" falls out of the key order.
 //    One pass over the surfel lanes feeds the old / new / composed views at once (the reference draws the whole
 //    buffer four times per render()).
-//  * transform feedback (ordered stream compaction)  ->  per-block counts + a single-block scan + an ordered scatter,
-//    so surfel order (and therefore every surfel index) is identical to the reference's.
+//  * transform feedback (ordered stream compaction)  ->  surfel order (and therefore every surfel index) is identical to
+//    the reference's. The surfel-indexed passes (update, tile extraction) publish per-block counts and 64-block group
+//    totals from their predicate kernel, and k_compact finds each block's offset from those; the pixel-indexed generation
+//    pass compacts in one kernel with a decoupled look-back.
 //  * surfels live as four float4 lanes (SoA), every pass streams only the lanes it needs with 128-bit accesses.
 #include "sb_gn.cuh"
 #include "sb_internal.cuh"
@@ -24,7 +26,7 @@ const char* kernel_name(int id) {
   static const char* names[K_COUNT] = {"fill_u64", "project_scatter", "preprocess_tile",
                                        "icp_jacobian", "gn_init", "icp_fused", "pose_products", "render_scatter",
                                        "render_resolve", "index_scatter", "radius", "update_surfels", "gen_surfels",
-                                       "extract_flags", "scan_blocks", "compact_scatter", "aos_to_soa", "soa_to_aos", "icp_post"};
+                                       "extract_flags", "compact_scatter", "aos_to_soa", "soa_to_aos", "icp_post"};
   return (id >= 0 && id < K_COUNT) ? names[id] : "?";
 }
 
@@ -889,6 +891,17 @@ __device__ __forceinline__ bool submap_keep(const float* __restrict__ poses, flo
   return true;
 }
 
+// Epilogue of the predicate kernels of the surfel-indexed passes, called by every thread of the block: two-level counts, so
+// that k_compact finds a block's output offset from <= 64 group totals + <= 63 block counts -- no scan pass. The
+// kGroupCounts totals of 64 blocks each must be zero before the predicate kernel runs.
+__device__ __forceinline__ void publish_block_count(bool kept, uint32_t* block_counts, uint32_t* group_counts) {
+  const int cnt = __syncthreads_count(kept ? 1 : 0);
+  if (threadIdx.x == 0) {
+    block_counts[blockIdx.x] = (uint32_t)cnt;
+    if (cnt) atomicAdd(group_counts + (blockIdx.x >> 6), (uint32_t)cnt);
+  }
+}
+
 struct UpdateArgs {
   Mat4 pose;               // current sensor pose (by value: no upload on the critical path)
   Mat4 inv_pose;
@@ -1044,13 +1057,8 @@ __global__ void __launch_bounds__(kThreads) k_update_surfels(KParams kp, SurfelP
     tmp.p3[k] = o3;
     keep[k] = kept ? 1 : 0;
   }
-  int cnt = __syncthreads_count(kept ? 1 : 0);
-  if (threadIdx.x == 0) {
-    block_counts[blockIdx.x] = (uint32_t)cnt;
-    // two-level counts: the ordered compaction that follows finds a block's output offset from <= 64 group totals + <= 63
-    // block counts -- no scan pass (group totals are cleared by the per-pixel prologue of the map update)
-    if (cnt) atomicAdd(group_counts + (blockIdx.x >> 6), (uint32_t)cnt);
-  }
+  // (group totals are cleared by the per-pixel prologue of the map update)
+  publish_block_count(kept, block_counts, group_counts);
 }
 
 // K6d + K6e in ONE pass: new surfels are appended in x-major pixel order behind the updated ones
@@ -1117,7 +1125,8 @@ __global__ void __launch_bounds__(kThreads) k_gen_compact(KParams kp, FrameDev f
 __global__ void __launch_bounds__(kThreads) k_extract_flags(SurfelPlanes s, const uint32_t* __restrict__ n_dev,
                                                            const float* __restrict__ poses, float2 center, float extent,
                                                            uint8_t* __restrict__ keep,
-                                                           uint32_t* __restrict__ block_counts) {
+                                                           uint32_t* __restrict__ block_counts,
+                                                           uint32_t* __restrict__ group_counts) {
   uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
   bool kept = false;
   if (k < *n_dev) {
@@ -1128,105 +1137,30 @@ __global__ void __launch_bounds__(kThreads) k_extract_flags(SurfelPlanes s, cons
     kept = !(fabsf(w.x - center.x) > extent || fabsf(w.y - center.y) > extent);
     keep[k] = kept ? 1 : 0;
   }
-  int cnt = __syncthreads_count(kept ? 1 : 0);
-  if (threadIdx.x == 0) block_counts[blockIdx.x] = (uint32_t)cnt;
+  publish_block_count(kept, block_counts, group_counts);
 }
 
-// ------------------------------------------------------------------------------------------------------------
-// ordered compaction (transform feedback semantics): block_counts[b] hold the kept items of block b (256 items)
-// ------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(1024) k_scan_blocks(const uint32_t* __restrict__ counts, uint32_t* __restrict__ offsets,
-                                                      const uint32_t* __restrict__ n_dev, uint32_t n_fixed,
-                                                      const uint32_t* __restrict__ base_dev, uint32_t cap,
-                                                      uint32_t* __restrict__ count_out,
-                                                      uint32_t* __restrict__ kept_out) {
-  __shared__ uint32_t warp_tot[32];
-  __shared__ uint32_t s_total;
-  uint32_t n = n_dev ? *n_dev : n_fixed;
-  uint32_t nblocks = (n + kThreads - 1) / kThreads;
-  uint32_t per = (nblocks + 1023) / 1024;
-  uint32_t b0 = threadIdx.x * per, b1 = min(b0 + per, nblocks);
-  uint32_t local = 0;
-  for (uint32_t b = b0; b < b1; ++b) local += counts[b];
-  // block-wide exclusive scan of `local`
-  uint32_t v = local;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    uint32_t u = __shfl_up_sync(0xffffffffu, v, o);
-    if (lane >= o) v += u;
-  }
-  if (lane == 31) warp_tot[warp] = v;
-  __syncthreads();
-  if (warp == 0) {
-    uint32_t w = warp_tot[lane];
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      uint32_t u = __shfl_up_sync(0xffffffffu, w, o);
-      if (lane >= o) w += u;
-    }
-    warp_tot[lane] = w;  // inclusive
-    if (lane == 31) s_total = w;
-  }
-  __syncthreads();
-  uint32_t excl = (v - local) + (warp > 0 ? warp_tot[warp - 1] : 0u);
-  uint32_t run = excl;
-  for (uint32_t b = b0; b < b1; ++b) {
-    offsets[b] = run;
-    run += counts[b];
-  }
-  if (threadIdx.x == 0) {
-    uint32_t base = base_dev ? *base_dev : 0u;
-    uint32_t tot = base + s_total;
-    if (kept_out) *kept_out = s_total;
-    *count_out = tot < cap ? tot : cap;
-  }
-}
-
-__global__ void __launch_bounds__(kThreads) k_compact_scatter(SurfelPlanes src, const uint8_t* __restrict__ keep,
-                                                             const uint32_t* __restrict__ offsets,
-                                                             const uint32_t* __restrict__ n_dev, uint32_t n_fixed,
-                                                             SurfelPlanes dst, const uint32_t* __restrict__ base_dev,
-                                                             uint32_t cap, uint32_t rel_cap) {
-  __shared__ uint32_t warp_cnt[kThreads / 32];
-  uint32_t n = n_dev ? *n_dev : n_fixed;
-  uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
-  bool kept = (k < n) && keep[k];
-  unsigned m = __ballot_sync(0xffffffffu, kept);
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  if (lane == 0) warp_cnt[warp] = __popc(m);
-  __syncthreads();
-  uint32_t before = 0;
-  for (int w = 0; w < warp; ++w) before += warp_cnt[w];
-  if (!kept) return;
-  uint32_t rank = before + __popc(m & ((1u << lane) - 1u));
-  uint32_t base = base_dev ? *base_dev : 0u;
-  uint32_t rel = offsets[blockIdx.x] + rank;
-  uint32_t d = base + rel;
-  if (d >= cap || rel >= rel_cap) return;  // transform feedback drops what does not fit
-  dst.p0[d] = src.p0[k];
-  dst.p1[d] = src.p1[k];
-  dst.p2[d] = src.p2[k];
-  dst.p3[d] = src.p3[k];
-}
-
-// Ordered compaction of the update pass without a scan kernel: block b's offset = sum of the group totals before its
-// group (<= 64 for 4M surfels) + the counts of the earlier blocks of its own group (<= 63), summed by one warp.
-// The last block also publishes the totals (S' = base of the new surfels, kept count).
-__global__ void __launch_bounds__(kThreads) k_compact_update(SurfelPlanes src, const uint8_t* __restrict__ keep,
-                                                            const uint32_t* __restrict__ block_counts,
-                                                            const uint32_t* __restrict__ group_counts,
-                                                            const uint32_t* __restrict__ n_dev, SurfelPlanes dst, uint32_t cap,
-                                                            uint32_t* __restrict__ count_out,
-                                                            uint32_t* __restrict__ kept_out) {
+// Ordered compaction (transform feedback semantics) of a surfel-indexed pass without a scan kernel: block b's offset =
+// sum of the group totals before its group (<= 64 for 4M surfels) + the counts of the earlier blocks of its own group
+// (<= 63), summed by one warp. The kept item of relative rank rel goes to dst[base + rel] iff rel < rel_cap and
+// base + rel < cap (transform feedback drops what does not fit), with base = *base_dev (0 if null; base <= cap).
+// The last block publishes out[0] = base + number written (the end of the written range), out[1] = number kept.
+__global__ void __launch_bounds__(kThreads) k_compact(SurfelPlanes src, const uint8_t* __restrict__ keep,
+                                                     const uint32_t* __restrict__ block_counts,
+                                                     const uint32_t* __restrict__ group_counts,
+                                                     const uint32_t* __restrict__ n_dev, SurfelPlanes dst,
+                                                     const uint32_t* __restrict__ base_dev, uint32_t cap, uint32_t rel_cap,
+                                                     uint32_t* __restrict__ out) {
   __shared__ uint32_t warp_cnt[kThreads / 32];
   __shared__ uint32_t s_offset;
   const uint32_t n = *n_dev;
   const uint32_t nblocks = (n + kThreads - 1) / kThreads;
+  const uint32_t base = base_dev ? *base_dev : 0u;
+  const uint32_t lim = min(rel_cap, cap - base);  // relative ranks below lim are written
   if (blockIdx.x >= nblocks) {
     if (nblocks == 0 && blockIdx.x == 0 && threadIdx.x == 0) {  // empty map
-      *count_out = 0;
-      if (kept_out) *kept_out = 0;
+      out[0] = base;
+      out[1] = 0;
     }
     return;
   }
@@ -1248,62 +1182,44 @@ __global__ void __launch_bounds__(kThreads) k_compact_update(SurfelPlanes src, c
   for (int w = 0; w < warp; ++w) before += warp_cnt[w];
   if (blockIdx.x == nblocks - 1 && threadIdx.x == 0) {
     const uint32_t total = s_offset + block_counts[blockIdx.x];
-    *count_out = total < cap ? total : cap;
-    if (kept_out) *kept_out = total;
+    out[0] = base + min(total, lim);
+    out[1] = total;
   }
   if (!kept) return;
-  const uint32_t d = s_offset + before + __popc(m & ((1u << lane) - 1u));
-  if (d >= cap) return;  // transform feedback drops what does not fit
+  const uint32_t rel = s_offset + before + __popc(m & ((1u << lane) - 1u));
+  if (rel >= lim) return;
+  const uint32_t d = base + rel;
   dst.p0[d] = src.p0[k];
   dst.p1[d] = src.p1[k];
   dst.p2[d] = src.p2[k];
   dst.p3[d] = src.p3[k];
 }
 
-void launch_compact_update(const Launch& L, SurfelPlanes src, const uint8_t* keep, const uint32_t* block_counts,
-                           const uint32_t* group_counts, const uint32_t* n_dev, uint32_t n_upper, SurfelPlanes dst,
-                           uint32_t cap, uint32_t* count_out, uint32_t* kept_out) {
+void launch_compact(const Launch& L, SurfelPlanes src, const uint8_t* keep, const uint32_t* block_counts,
+                    const uint32_t* group_counts, const uint32_t* n_dev, uint32_t n_upper, SurfelPlanes dst,
+                    const uint32_t* base_dev, uint32_t cap, uint32_t rel_cap, uint32_t* out) {
   uint32_t blocks = (n_upper + kThreads - 1) / kThreads;
   if (blocks == 0) blocks = 1;
   {
     ScopedKernel sk(L, K_COMPACT_SCATTER);
-    k_compact_update<<<blocks, kThreads, 0, L.stream>>>(src, keep, block_counts, group_counts, n_dev, dst, cap, count_out,
-                                                       kept_out);
+    k_compact<<<blocks, kThreads, 0, L.stream>>>(src, keep, block_counts, group_counts, n_dev, dst, base_dev, cap, rel_cap,
+                                                 out);
   }
 }
 
 // ---- submap tile cache in HBM: a leaving tile is compacted straight into a device-resident pool (the reference
-// downloads it to host RAM, SurfelMap.cpp:708-742). rec = {base, count} of the tile inside the pool.
-__global__ void k_pool_alloc(uint2* __restrict__ rec, uint32_t* __restrict__ pool_top, uint32_t pool_cap) {
-  uint32_t base = *pool_top, cnt = rec->y;
-  if (base > pool_cap) base = pool_cap;
-  if (cnt > pool_cap - base) {  // pool exhausted: the tail of the tile is lost -- counted in pool_top[1], which the host
-    pool_top[1] += cnt - (pool_cap - base);  // reads with the tile records and reports (sb_get_statistics[12], sb_last_error)
-    cnt = pool_cap - base;
-  }
-  rec->x = base;
-  rec->y = cnt;
-  *pool_top = base + cnt;
-}
-
+// downloads it to host RAM, SurfelMap.cpp:708-742). Slot s of the pool starts where slot s - 1 ends (slot 0 at 0);
+// rec[s] = {end of slot s in the pool, surfels of the tile}.
 void launch_extract_to_pool(const Launch& L, SurfelPlanes map, const uint32_t* n_dev, uint32_t n_upper, const float* poses,
-                            float2 center, float extent, uint8_t* keep, uint32_t* block_counts, uint32_t* block_offsets,
-                            SurfelPlanes pool, uint32_t pool_cap, uint32_t* pool_top, uint2* rec, uint32_t tile_cap) {
-  launch_extract_flags(L, map, n_dev, n_upper, poses, center, extent, keep, block_counts);
-  {
-    ScopedKernel sk(L, K_SCAN_BLOCKS);
-    k_scan_blocks<<<1, 1024, 0, L.stream>>>(block_counts, block_offsets, n_dev, n_upper, nullptr, tile_cap, &rec->y, nullptr);
+                            float2 center, float extent, uint8_t* keep, uint32_t* block_counts, uint32_t* group_counts,
+                            SurfelPlanes pool, uint32_t pool_cap, uint2* rec, uint32_t slot, uint32_t tile_cap) {
+  if (n_upper > 0) {
+    ScopedKernel sk(L, K_EXTRACT_FLAGS);
+    k_extract_flags<<<(n_upper + kThreads - 1) / kThreads, kThreads, 0, L.stream>>>(map, n_dev, poses, center, extent, keep,
+                                                                                 block_counts, group_counts);
   }
-  {
-    ScopedKernel sk(L, K_SCAN_BLOCKS);
-    k_pool_alloc<<<1, 1, 0, L.stream>>>(rec, pool_top, pool_cap);
-  }
-  if (n_upper == 0) return;
-  {
-    ScopedKernel sk(L, K_COMPACT_SCATTER);
-    k_compact_scatter<<<(n_upper + kThreads - 1) / kThreads, kThreads, 0, L.stream>>>(
-        map, keep, block_offsets, n_dev, n_upper, pool, &rec->x, pool_cap, tile_cap);
-  }
+  launch_compact(L, map, keep, block_counts, group_counts, n_dev, n_upper, pool, slot ? &rec[slot - 1].x : nullptr,
+                 pool_cap, tile_cap, &rec[slot].x);
 }
 
 void launch_update_surfels(const Launch& L, const KParams& kp, SurfelPlanes src, SurfelPlanes tmp, const uint32_t* n_dev,
@@ -1334,16 +1250,6 @@ void launch_gen_compact(const Launch& L, const KParams& kp, FrameDev frame, cons
     k_gen_compact<<<(P + kThreads - 1) / kThreads, kThreads, 0, L.stream>>>(kp, frame, radius_map, integrated, poses,
                                                                            timestamp, submap_center, submap_extent, map,
                                                                            lb, cap, counts);
-  }
-}
-
-void launch_extract_flags(const Launch& L, SurfelPlanes s, const uint32_t* n_dev, uint32_t n_upper, const float* poses,
-                          float2 center, float extent, uint8_t* keep, uint32_t* block_counts) {
-  if (n_upper == 0) return;
-  {
-    ScopedKernel sk(L, K_EXTRACT_FLAGS);
-    k_extract_flags<<<(n_upper + kThreads - 1) / kThreads, kThreads, 0, L.stream>>>(s, n_dev, poses, center, extent, keep,
-                                                                                 block_counts);
   }
 }
 

@@ -55,6 +55,12 @@ def test_map_update_on_an_image_under_256_pixels():
     assert _child(["tests/test_gpu_shapes.py"], "test_map_updates_on_an_image_under_256_pixels") == 1
 
 
+def test_submap_paging_on_the_cpu_executor():
+    """several tiles extracted per update, a tile over the 500 000-surfel extract cap and paging an empty map, each against
+    the oracle (tests/test_gpu_paging.py; the pool exhaustion case runs in the full tier)"""
+    assert _child(["tests/test_gpu_paging.py"], "not exhaustion") == 3
+
+
 @long_run
 def test_kernel_results_do_not_depend_on_the_execution_order():
     """CUDA promises no order between the lanes of a warp or the warps of a block outside its synchronisation primitives:
