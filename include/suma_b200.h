@@ -161,7 +161,9 @@ int sb_map_timestamp(sb_ctx* ctx, uint32_t* t);
 int sb_map_download(sb_ctx* ctx, sb_surfel* dst, uint32_t cap, uint32_t* n); /* SurfelMap::getAllSurfels */
 int sb_map_upload(sb_ctx* ctx, const sb_surfel* src, uint32_t n, uint32_t timestamp); /* test / restore hook */
 int sb_map_set_pose(sb_ctx* ctx, uint32_t t, const float pose[16]);
-/* intermediates of the last update (any pointer may be NULL): index map (id+1), radius map, integrated flags */
+/* intermediates of the last update (any pointer may be NULL): index map (id+1), radius map, integrated flags.
+   After sb_map_update the ids index the surfels in order (as sb_map_download returns them); after sb_process_scan they
+   are the map's physical slots, which may include slots of surfels removed by in-place updates (same relative order). */
 int sb_map_update_debug(sb_ctx* ctx, uint32_t* index_map, float* radius_map4, uint8_t* integrated,
                         uint32_t* n_updated, uint32_t* n_new);
 int sb_map_submap_origin(sb_ctx* ctx, int32_t* i, int32_t* j, uint32_t* pending);

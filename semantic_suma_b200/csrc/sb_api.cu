@@ -92,6 +92,9 @@ struct sb_ctx {
   // current surfels, updated (same index), generated (per pixel), extraction buffer: views into the *_mem allocations
   SurfelPlanes A{}, T{}, G{}, X{};
   DevPtr<float4> A_mem, T_mem, G_mem, X_mem;
+  // liveness byte per slot of A, valid below the physical end: set by every writer of a slot, cleared only by the
+  // in-place map update (a surfel it removes stays where it is, dead, until the next compaction)
+  DevPtr<uint8_t> live;
   DevPtr<uint8_t> keep;
   DevPtr<uint32_t> block_counts;
   DevPtr<unsigned long long> lb_desc;  // look-back descriptors of the single-pass compactions
@@ -112,7 +115,9 @@ struct sb_ctx {
   DevPtr<uint32_t> group_counts;  // kGroupCounts totals of the update pass / a tile extraction (64 blocks each)
   FramePtr f_old, f_new, f_comp;
   uint64_t frames_created = 0;
-  uint32_t n_host = 0;   // surfel count (exact; refreshed after every update)
+  uint32_t n_host = 0;   // physical end of the surfel slots (exact; refreshed after every update)
+  uint32_t n_holes = 0;  // dead slots below n_host: the map holds n_host - n_holes surfels
+  bool lazy_update = false;  // the map update in flight is the in-place one (its counts[5] is the new n_holes)
   uint32_t n_upper = 0;  // upper bound used for grid sizing while the exact count is still in flight
   uint32_t n_updated = 0, n_new = 0;
   uint32_t map_timestamp = 0;
@@ -268,7 +273,8 @@ void frame_written(sb_ctx* c, const sb_frame* f) {
 int reset_state(sb_ctx* c) {
   // SurfelMap::reset (SurfelMap.cpp:473-482) + the SurfelMapping members set up in its constructor
   c->map_version += 1;
-  c->n_host = 0; c->n_updated = 0; c->n_new = 0; c->map_timestamp = 0;
+  c->n_host = 0; c->n_holes = 0; c->lazy_update = false;
+  c->n_updated = 0; c->n_new = 0; c->map_timestamp = 0;
   c->origin_i = c->origin_j = 0;
   c->extraction.clear();
   c->tiles.clear();
@@ -344,6 +350,7 @@ int alloc_buffers(sb_ctx* c) {
   if ((r = alloc_planes(c, c->X_mem, &c->X, 16))) return r;
   if ((r = alloc_planes(c, c->pool_mem, &c->pool, kTilePoolCap))) return r;
   SB_CUDA(c, dev_alloc(c->d_tile_rec, (size_t)kMaxTileSlots * sizeof(uint2)));
+  SB_CUDA(c, dev_alloc(c->live, kMaxSurfels));
   SB_CUDA(c, dev_alloc(c->keep, kMaxSurfels));
   size_t nb = (kMaxSurfels + 127) / 128 + 16;  // blocks of the finest-grained surfel kernel
   SB_CUDA(c, dev_alloc(c->block_counts, nb * 4));
@@ -379,6 +386,8 @@ int alloc_buffers(sb_ctx* c) {
 }
 
 uint32_t n_grid(const sb_ctx* c) { return c->n_upper > c->n_host ? c->n_upper : c->n_host; }
+
+uint32_t n_live(const sb_ctx* c) { return c->n_host - c->n_holes; }
 
 int t_threshold(const sb_ctx* c) { return (int)(c->map_timestamp - kComposeAge); }  // SurfelMap.cpp:873 (Q9)
 
@@ -450,17 +459,17 @@ int render_full(sb_ctx* c, const float* pose_old, const float* pose_new, float c
     RenderTargets t{c->key_old, c->key_new, nullptr};
     int thr = t_threshold(c);
     if (same) {
-      launch_render_scatter(L, kp, c->A, c->res->counts, n_grid(c), c->Mtab_old, conf_thr, thr, 1, 1, 0, t);
+      launch_render_scatter(L, kp, c->A, c->res->counts, c->live, n_grid(c), c->Mtab_old, conf_thr, thr, 1, 1, 0, t);
     } else {
       RenderTargets to{c->key_old, nullptr, nullptr}, tn{nullptr, c->key_new, nullptr};
-      launch_render_scatter(L, kp, c->A, c->res->counts, n_grid(c), c->Mtab_old, conf_thr, thr, 1, 0, 0, to);
-      launch_render_scatter(L, kp, c->A, c->res->counts, n_grid(c), Mnew, conf_thr, thr, 0, 1, 0, tn);
+      launch_render_scatter(L, kp, c->A, c->res->counts, c->live, n_grid(c), c->Mtab_old, conf_thr, thr, 1, 0, 0, to);
+      launch_render_scatter(L, kp, c->A, c->res->counts, c->live, n_grid(c), Mnew, conf_thr, thr, 0, 1, 0, tn);
     }
     launch_render_resolve(L, kp, c->A, c->Mtab_old, Mnew, t, c->f_old->d, c->f_new->d, c->f_comp->d, out->d, null_frame(), 0, 0);
   } else {
     // SurfelMap.cpp:977-1017: one view with render_old_surfels = false, timestamp_threshold = 0, copied to old and new
     RenderTargets t{nullptr, c->key_new, nullptr};
-    launch_render_scatter(L, kp, c->A, c->res->counts, n_grid(c), c->Mtab_old, conf_thr, 0, 0, 1, 0, t);
+    launch_render_scatter(L, kp, c->A, c->res->counts, c->live, n_grid(c), c->Mtab_old, conf_thr, 0, 0, 1, 0, t);
     launch_render_resolve(L, kp, c->A, c->Mtab_old, c->Mtab_old, t, null_frame(), c->f_new->d, null_frame(), null_frame(),
                           null_frame(), 0, 0);
     SB_CUDA(c, cudaMemcpyAsync(c->f_old->base, c->f_new->base, Pm * 48, cudaMemcpyDeviceToDevice, c->stream));
@@ -486,7 +495,7 @@ int render_single(sb_ctx* c, const float* pose, float conf_thr, int which, const
   if (!table_ready) launch_pose_products(L, mat4_from(inv), inv_dev, c->poses, c->Mtab_old, pose_table_count(c));
   unsigned long long* key = which ? c->key_new : c->key_old;
   RenderTargets t{which ? nullptr : key, which ? key : nullptr, nullptr};
-  launch_render_scatter(L, kp, c->A, c->res->counts, n_grid(c), c->Mtab_old, conf_thr, t_threshold(c), which ? 0 : 1,
+  launch_render_scatter(L, kp, c->A, c->res->counts, c->live, n_grid(c), c->Mtab_old, conf_thr, t_threshold(c), which ? 0 : 1,
                         which ? 1 : 0, 0, t);
   // copy_to: lastModelFrame_->copy(*map_->newMapFrame()), SurfelMapping.cpp:407 (the semantic image is the stale one, Q4),
   // written by the same resolve pass
@@ -638,6 +647,10 @@ int icp_minimize_fetch(sb_ctx* c, double* pose_out, double* out48, int* iters, d
 // ---------------------------------------------------------------------------------------------------------
 // map update: SurfelMap::update, SurfelMap.cpp:492-584
 // ---------------------------------------------------------------------------------------------------------
+// The per-scan map update runs dense (update into T + compaction back into A) once the dead slots left by the in-place
+// updates reach this fraction of the physical end (1 / kDenseHoleFraction); DESIGN.md section 7 gives the measurements.
+constexpr uint32_t kDenseHoleFraction = 8;
+
 float2 submap_center(const sb_ctx* c, int32_t i, int32_t j) {  // submapIndex2center, SurfelMap.cpp:704-706
   return make_float2((float)(2.0 * i * c->p.submap_extent), (float)(2.0 * j * c->p.submap_extent));
 }
@@ -677,6 +690,26 @@ int refresh_tile_records(sb_ctx* c) {  // read back the records of the tiles ext
   return SB_OK;
 }
 
+// Moves the live surfels of a map with dead slots to the front, in order (A -> T, then the two sets swap roles): what
+// observers of the map and the operator-level update see, and what a tile that needs the room finds.
+int compact_map(sb_ctx* c) {
+  if (c->n_holes == 0) return SB_OK;
+  // the host's physical end is the one to compact: tile re-insertion raises it ahead of counts[0]
+  SB_CUDA(c, cudaMemcpyAsync(c->res->counts, &c->n_host, 4, cudaMemcpyHostToDevice, c->stream));
+  SB_CUDA(c, cudaMemsetAsync(c->group_counts, 0, kGroupCounts * 4, c->stream));
+  launch_compact_live(L_(c), c->A, c->res->counts, c->n_host, c->live, c->keep, c->block_counts, c->group_counts, c->T,
+                      c->res->counts + 6);
+  SB_CUDA(c, cudaStreamSynchronize(c->stream));  // (the copy above reads the member changed below)
+  std::swap(c->A, c->T);  // both are kMaxSurfels sets with the same lane pitch
+  std::swap(c->A_mem, c->T_mem);
+  c->n_host = n_live(c);
+  c->n_holes = 0;
+  c->n_upper = c->n_host;
+  SB_CUDA(c, cudaMemcpyAsync(c->res->counts, &c->n_host, 4, cudaMemcpyHostToDevice, c->stream));
+  SB_CUDA(c, cudaStreamSynchronize(c->stream));  // the copy reads a member of the context: keep it ordered
+  return SB_OK;
+}
+
 int append_tiles(sb_ctx* c, int32_t i0, int32_t j0, int di, int dj) {  // SurfelMap.cpp:769-780
   const int dim = c->p.submap_dimension;
   int r;
@@ -686,6 +719,8 @@ int append_tiles(sb_ctx* c, int32_t i0, int32_t j0, int di, int dj) {  // Surfel
     if (it == c->tiles.end()) continue;  // submapCache_[idx] of a tile never extracted: empty
     if (!it->second.known && (r = refresh_tile_records(c))) return r;
     const DevTile& t = it->second;
+    // the reference's map has no dead slots: a tile that does not fit behind them fits (or is cut) after compaction
+    if (t.count > kMaxSurfels - c->n_host && (r = compact_map(c))) return r;
     uint32_t room = kMaxSurfels - c->n_host;
     uint32_t n = t.count < room ? t.count : room;
     if (n == 0) continue;
@@ -693,6 +728,7 @@ int append_tiles(sb_ctx* c, int32_t i0, int32_t j0, int di, int dj) {  // Surfel
     for (size_t lane = 0; lane < 4; ++lane)
       SB_CUDA(c, cudaMemcpyAsync(c->A.p0 + lane * kMaxSurfels + c->n_host, c->pool.p0 + lane * kTilePoolCap + t.base,
                                  (size_t)n * 16, cudaMemcpyDeviceToDevice, c->stream));
+    SB_CUDA(c, cudaMemsetAsync(c->live + c->n_host, 1, n, c->stream));
     c->n_host += n;
     c->n_upper = c->n_host;
     appended = true;
@@ -716,8 +752,8 @@ int extract_surfels(sb_ctx* c, bool partially) {
     uint32_t slot = c->n_slots++;
     // extractions can follow each other with no per-pixel prologue in between to clear the group totals
     SB_CUDA(c, cudaMemsetAsync(c->group_counts, 0, kGroupCounts * 4, c->stream));
-    launch_extract_to_pool(L, c->A, c->res->counts, c->n_host, c->poses, ctr, c->p.submap_extent, c->keep, c->block_counts,
-                           c->group_counts, c->pool, kTilePoolCap, c->d_tile_rec, slot, kExtractCap);
+    launch_extract_to_pool(L, c->A, c->res->counts, c->live, c->n_host, c->poses, ctr, c->p.submap_extent, c->keep,
+                           c->block_counts, c->group_counts, c->pool, kTilePoolCap, c->d_tile_rec, slot, kExtractCap);
     DevTile t;
     t.slot = slot;
     t.known = false;
@@ -764,6 +800,8 @@ int map_update(sb_ctx* c, const float* pose, const sb_frame* frame, const Mat4* 
   const bool deferred = pose_dev != nullptr;
   int r;
   float inv_pose[16] = {0}, pose_h[16] = {0};
+  // the operator-level update works on the compacted map: its index map (sb_map_update_debug) indexes the surfels in order
+  if (!deferred && (r = compact_map(c))) return r;
   if (!deferred) {
     if (c->map_timestamp < kMaxPoses) {
       if ((r = set_pose_entry(c, c->map_timestamp, pose))) return r;  // SurfelMap.cpp:494-495
@@ -777,26 +815,37 @@ int map_update(sb_ctx* c, const float* pose, const sb_frame* frame, const Mat4* 
   // when the frame is the one it produced
   if (!(c->prepped_for_update && frame == c->cur)) launch_radius(L, kp, frame->d, c->radius_map, c->key_index, c->integrated, c->group_counts);
   c->prepped_for_update = false;
-  launch_index_scatter(L, kp, c->A, c->res->counts, n_grid(c), c->Mtab_old, c->key_index);
+  launch_index_scatter(L, kp, c->A, c->res->counts, c->live, n_grid(c), c->Mtab_old, c->key_index);
   // K6c + K6e predicate
   float2 ctr = submap_center(c, c->origin_i, c->origin_j);
   float extent = 2.0f * c->p.submap_dimension * c->p.submap_extent + c->p.submap_extent;  // :674
   if (c->p.partial_extraction && !c->extraction.empty()) extent += 2.0f * c->p.submap_extent;  // :677
-  // K6c + K6e predicate, then ordered compaction back into the map lanes: counts[1] = S', counts[2] = kept.
+  // In place (lazy) or dense, decided from what the host already knows (no extra synchronisation); DESIGN.md section 7.
+  // Dense when the dead slots reach 1 / kDenseHoleFraction of the physical end, when the new surfels could hit the capacity
+  // behind the dead slots (k_gen_compact must cut exactly where the compacted map would), and at the operator level.
+  const uint32_t n = n_grid(c);
+  const bool lazy = deferred && n > 0 && (uint64_t)c->n_holes * kDenseHoleFraction < n &&
+                    (uint64_t)n + Pd <= kMaxSurfels;
+  c->lazy_update = lazy;
+  // Dense: K6c + K6e predicate into T, then ordered compaction back into the map lanes: counts[1] = S', counts[2] = kept.
   // (A single-pass variant with decoupled look-back was measured twice and loses: round 1 with a 32-wide chain, round 2
   // with 256-wide windows that stop at the nearest inclusive prefix -- 80.2 us against 48.8 + 23.8 us for the two
   // passes at S = 1.2 M: the ~400 resident blocks finish their heavy per-surfel work together, hold their SM slots
   // through several dependent L2 round trips and only then issue their writes.)
-  launch_update_surfels(L, kp, c->A, c->T, c->res->counts, n_grid(c), mat4_from(pose_h), mat4_from(inv_pose), pose_dev,
+  // Lazy: the changed lanes are stored in place and removed surfels marked dead; counts[1] = physical end, and the
+  // generation pass below writes [2] = kept and [5] = dead slots from the update's group totals.
+  launch_update_surfels(L, kp, lazy, c->A, c->T, c->res->counts, n, mat4_from(pose_h), mat4_from(inv_pose), pose_dev,
                         inv_dev, c->poses, c->poses_inv, c->key_index, c->radius_map, frame->d, (int)c->map_timestamp,
-                        ctr, extent, c->integrated, c->keep, c->block_counts, c->group_counts);
-  launch_compact(L, c->T, c->keep, c->block_counts, c->group_counts, c->res->counts, n_grid(c), c->A, nullptr, kMaxSurfels,
-                 kMaxSurfels, c->res->counts + 1);
-  // K6d + K6e: new surfels appended behind the updated ones; counts[0] = new map size, counts[3] = new surfels
+                        ctr, extent, c->integrated, c->live, c->keep, c->block_counts, c->group_counts);
+  if (!lazy)
+    launch_compact(L, c->T, c->keep, c->block_counts, c->group_counts, c->res->counts, n, c->A, c->live, nullptr,
+                   kMaxSurfels, kMaxSurfels, c->res->counts + 1);
+  // K6d + K6e: new surfels appended behind counts[1]; counts[0] = new physical end, counts[3] = new surfels
   c->lb_gen = (c->lb_gen + 1) & 0x3fffffffu;
   if (c->lb_gen == 0) c->lb_gen = 1;
   launch_gen_compact(L, kp, frame->d, c->radius_map, c->integrated, c->poses, (int)c->map_timestamp, ctr, extent, c->A,
-                     c->lb_desc, c->lb_ticket, c->lb_gen, kMaxSurfels, c->res->counts);
+                     c->live, lazy ? c->group_counts.get() : nullptr, c->lb_desc, c->lb_ticket, c->lb_gen, kMaxSurfels,
+                     c->res->counts);
   uint64_t up = (uint64_t)n_grid(c) + Pd;  // the map can grow by at most one surfel per pixel
   c->n_upper = up > kMaxSurfels ? kMaxSurfels : (uint32_t)up;
   if (deferred) {
@@ -806,6 +855,7 @@ int map_update(sb_ctx* c, const float* pose, const sb_frame* frame, const Mat4* 
   uint32_t cnt[4];
   if ((r = fetch_counts(c, cnt, 4))) return r;
   c->n_host = cnt[0];
+  c->n_holes = 0;  // (dense)
   c->n_upper = cnt[0];
   c->n_updated = cnt[2];
   c->n_new = cnt[3];
@@ -902,8 +952,8 @@ int render_composed_internal(sb_ctx* c, const float* pose_old, const float* pose
   RenderTargets t{nullptr, nullptr, c->key_comp};
   int thr = t_threshold(c);
   // GL_LEQUAL (SurfelMap.cpp:1126), old then new without clearing (:1146-1152); COLOR2 not attached (Q4)
-  launch_render_scatter(L, kp, c->A, c->res->counts, n_grid(c), c->Mtab_old, conf_thr, thr, 1, 0, 1, t);
-  launch_render_scatter(L, kp, c->A, c->res->counts, n_grid(c), c->Mtab_new, conf_thr, thr, 0, 1, 1, t);
+  launch_render_scatter(L, kp, c->A, c->res->counts, c->live, n_grid(c), c->Mtab_old, conf_thr, thr, 1, 0, 1, t);
+  launch_render_scatter(L, kp, c->A, c->res->counts, c->live, n_grid(c), c->Mtab_new, conf_thr, thr, 0, 1, 1, t);
   launch_render_resolve(L, kp, c->A, c->Mtab_old, c->Mtab_new, t, null_frame(), null_frame(), c->f_comp->d, null_frame(),
                         null_frame(), 1, 1);
   SB_CUDA(c, cudaGetLastError());
@@ -1453,7 +1503,7 @@ int sb_map_set_pose(sb_ctx* c, uint32_t t, const float pose[16]) {
 }
 int sb_map_size(sb_ctx* c, uint32_t* n) {
   if (!c || !n) return SB_ERR_INVALID;
-  *n = c->n_host;
+  *n = n_live(c);  // (no compaction: dead slots cost the readers nothing but a byte)
   return SB_OK;
 }
 int sb_map_timestamp(sb_ctx* c, uint32_t* t) {
@@ -1464,6 +1514,8 @@ int sb_map_timestamp(sb_ctx* c, uint32_t* t) {
 int sb_map_download(sb_ctx* c, sb_surfel* dst, uint32_t cap, uint32_t* n) {
   if (!c || (!dst && cap)) return SB_ERR_INVALID;
   cudaSetDevice(c->device);
+  int r = compact_map(c);
+  if (r) return r;
   uint32_t k = c->n_host < cap ? c->n_host : cap;
   if (n) *n = k;
   if (k == 0) return SB_OK;
@@ -1480,8 +1532,10 @@ int sb_map_upload(sb_ctx* c, const sb_surfel* src, uint32_t n, uint32_t timestam
   if (n) {
     SB_CUDA(c, cudaMemcpyAsync(c->T.p0, src, (size_t)n * 64, cudaMemcpyHostToDevice, c->stream));
     launch_aos_to_soa(L_(c), reinterpret_cast<const sb_surfel*>(c->T.p0), c->A, 0, n);
+    SB_CUDA(c, cudaMemsetAsync(c->live, 1, n, c->stream));
   }
   c->n_host = n;
+  c->n_holes = 0;  // (overwritten: nothing to compact)
   c->n_upper = n;
   c->map_timestamp = timestamp;
   c->map_version += 1;
@@ -1567,12 +1621,15 @@ int sb_process_scan(sb_ctx* c, const float* pts4, const float* labels, const flo
   SB_CUDA(c, cudaStreamSynchronize(c->stream));
   const double t_synced = now_s();
   SB_CUDA(c, cudaGetLastError());
-  if (rb.pose.gn_error) return gn_fail(c);
-  if (!loop_ran) absorb_pose_block(c, rb, had_icp);  // (the loop-closure step has already done it, and chose currentPose_old_)
+  // the map update has run on the device even when the scan fails below: the host's counts follow it, so that a later
+  // compaction (download) covers the map as it is
   c->n_host = rb.counts[0];
+  c->n_holes = c->lazy_update ? rb.counts[5] : 0;
   c->n_upper = rb.counts[0];
   c->n_updated = rb.counts[2];
   c->n_new = rb.counts[3];
+  if (rb.pose.gn_error) return gn_fail(c);
+  if (!loop_ran) absorb_pose_block(c, rb, had_icp);  // (the loop-closure step has already done it, and chose currentPose_old_)
   const Mat4 P_cur = rb.pose.P_cur;
   if (t_map < kMaxPoses) {  // host mirror of the pose table entry written by k_pose_finalize
     memcpy(&c->h_poses[16 * (size_t)t_map], P_cur.m, 64);
@@ -1587,7 +1644,7 @@ int sb_process_scan(sb_ctx* c, const float* pts4, const float* labels, const flo
     if ((r = update_active_submaps(c, P_cur.m))) return r;
     if (c->n_host != n0 && p.render_after_update && (r = render_full(c, P_cur.m, P_cur.m, ct2, c->cur_model))) return r;
   }
-  c->stats[7] = c->n_host;
+  c->stats[7] = n_live(c);
   // The reference's three stage timers (preprocessing / icp / mapping) have no meaning here -- the stages overlap on
   // the stream; the slots carry the host-side split of the call instead: enqueue, wait for the device, bookkeeping.
   const double t_end = now_s();

@@ -120,7 +120,10 @@ struct ResultBlock {
   char pad0[4096 - sizeof(PoseDev)];
   long long sums[64];                 // raw sums of a Jacobian pass (the first 32; the scan's statistics pass)
   char pad1[8192 - 4096 - 64 * sizeof(long long)];
-  uint32_t counts[16];  // [0] n surfels, [1] n after update (base for new), [2] kept updated, [3] kept new, [4] extracted
+  // [0] physical end of the surfel slots, [1] physical end after the update (base for new), [2] kept updated,
+  // [3] kept new, [4] extracted, [5] dead slots below [1] after an in-place update, [6] / [7] end of the written range /
+  // number kept of a compaction of the map (not read back)
+  uint32_t counts[16];
 };
 static_assert(offsetof(ResultBlock, sums) == 4096, "result block layout");
 static_assert(offsetof(ResultBlock, counts) == 8192, "result block layout");
@@ -249,37 +252,48 @@ struct RenderTargets {
 };
 void launch_pose_products(const Launch& L, const Mat4& A, const Mat4* A_dev, const float* poses, float* out,
                           uint32_t count);
-void launch_render_scatter(const Launch& L, const KParams& kp, SurfelPlanes s, const uint32_t* n_dev, uint32_t n_upper,
-                           const float* M, float conf_thr, int t_thr, int emit_old, int emit_new, int lequal,
-                           RenderTargets t);
+// Surfel slots [0, counts[0]) of the map; a slot whose liveness byte is 0 holds a surfel removed by an in-place update.
+void launch_render_scatter(const Launch& L, const KParams& kp, SurfelPlanes s, const uint32_t* n_dev, const uint8_t* live,
+                           uint32_t n_upper, const float* M, float conf_thr, int t_thr, int emit_old, int emit_new,
+                           int lequal, RenderTargets t);
 void launch_render_resolve(const Launch& L, const KParams& kp, SurfelPlanes s, const float* M_old, const float* M_new,
                            RenderTargets t, FrameDev f_old, FrameDev f_new, FrameDev f_comp, FrameDev f_out,
                            FrameDev f_copy, int keep_semantic, int lequal);
-void launch_index_scatter(const Launch& L, const KParams& kp, SurfelPlanes s, const uint32_t* n_dev, uint32_t n_upper,
-                          const float* M, unsigned long long* keys);
+void launch_index_scatter(const Launch& L, const KParams& kp, SurfelPlanes s, const uint32_t* n_dev, const uint8_t* live,
+                          uint32_t n_upper, const float* M, unsigned long long* keys);
 void launch_radius(const Launch& L, const KParams& kp, FrameDev frame, float4* radius_map, unsigned long long* index_keys,
                    uint8_t* integrated, uint32_t* group_counts);
 // ordered compaction of a surfel-indexed pass: items flagged in keep[0..n) of src go to dst[base..) in order, base =
-// *base_dev (0 if null); out[0] = end of the written range, out[1] = number of items kept
+// *base_dev (0 if null); out[0] = end of the written range, out[1] = number of items kept; dst_live (or null): liveness
+// bytes of the destination, set for every slot written
 void launch_compact(const Launch& L, SurfelPlanes src, const uint8_t* keep, const uint32_t* block_counts,
                     const uint32_t* group_counts, const uint32_t* n_dev, uint32_t n_upper, SurfelPlanes dst,
-                    const uint32_t* base_dev, uint32_t cap, uint32_t rel_cap, uint32_t* out);
-void launch_update_surfels(const Launch& L, const KParams& kp, SurfelPlanes src, SurfelPlanes tmp, const uint32_t* n_dev,
-                           uint32_t n_upper, const Mat4& pose, const Mat4& inv_pose, const Mat4* pose_dev,
-                           const Mat4* inv_pose_dev, const float* poses,
+                    uint8_t* dst_live, const uint32_t* base_dev, uint32_t cap, uint32_t rel_cap, uint32_t* out);
+// the live surfels of src, in order, to dst[0..); `live` is read for src and then set for dst. The group totals must be
+// zero; out must not alias *n_dev.
+void launch_compact_live(const Launch& L, SurfelPlanes src, const uint32_t* n_dev, uint32_t n_upper, uint8_t* live,
+                         uint8_t* keep, uint32_t* block_counts, uint32_t* group_counts, SurfelPlanes dst, uint32_t* out);
+// lazy = false: updated records into tmp + keep bytes for launch_compact; lazy = true: in place in src, removed surfels
+// marked dead in `live`, counts[1] = physical end
+void launch_update_surfels(const Launch& L, const KParams& kp, bool lazy, SurfelPlanes src, SurfelPlanes tmp,
+                           uint32_t* counts, uint32_t n_upper, const Mat4& pose, const Mat4& inv_pose,
+                           const Mat4* pose_dev, const Mat4* inv_pose_dev, const float* poses,
                            const float* poses_inv, const unsigned long long* index_keys, const float4* radius_map,
                            FrameDev frame, int timestamp, float2 submap_center, float submap_extent,
-                           uint8_t* integrated, uint8_t* keep, uint32_t* block_counts, uint32_t* group_counts);
-// single-pass update / generate with in-place ordered compaction (decoupled look-back)
+                           uint8_t* integrated, uint8_t* live, uint8_t* keep, uint32_t* block_counts,
+                           uint32_t* group_counts);
+// single-pass update / generate with in-place ordered compaction (decoupled look-back), appended behind counts[1];
+// lazy_groups (the group totals of an in-place update, or null): counts[2] = their sum, counts[5] = counts[1] - sum
 void launch_gen_compact(const Launch& L, const KParams& kp, FrameDev frame, const float4* radius_map,
                         const uint8_t* integrated, const float* poses, int timestamp, float2 submap_center,
-                        float submap_extent, SurfelPlanes map, unsigned long long* desc, uint32_t* ticket, uint32_t gen,
-                        uint32_t cap, uint32_t* counts);
-// the surfels of one submap tile, in order, into pool slot `slot`: rec[slot] = {end of the slot in the pool, surfels of
-// the tile}; slot s starts at the end of slot s - 1. The group totals must be zero.
-void launch_extract_to_pool(const Launch& L, SurfelPlanes map, const uint32_t* n_dev, uint32_t n_upper, const float* poses,
-                            float2 center, float extent, uint8_t* keep, uint32_t* block_counts, uint32_t* group_counts,
-                            SurfelPlanes pool, uint32_t pool_cap, uint2* rec, uint32_t slot, uint32_t tile_cap);
+                        float submap_extent, SurfelPlanes map, uint8_t* live, const uint32_t* lazy_groups,
+                        unsigned long long* desc, uint32_t* ticket, uint32_t gen, uint32_t cap, uint32_t* counts);
+// the live surfels of one submap tile, in order, into pool slot `slot`: rec[slot] = {end of the slot in the pool, surfels
+// of the tile}; slot s starts at the end of slot s - 1. The group totals must be zero.
+void launch_extract_to_pool(const Launch& L, SurfelPlanes map, const uint32_t* n_dev, const uint8_t* live, uint32_t n_upper,
+                            const float* poses, float2 center, float extent, uint8_t* keep, uint32_t* block_counts,
+                            uint32_t* group_counts, SurfelPlanes pool, uint32_t pool_cap, uint2* rec, uint32_t slot,
+                            uint32_t tile_cap);
 void launch_aos_to_soa(const Launch& L, const sb_surfel* aos, SurfelPlanes s, uint32_t offset, uint32_t n);
 void launch_soa_to_aos(const Launch& L, SurfelPlanes s, sb_surfel* aos, uint32_t n);
 

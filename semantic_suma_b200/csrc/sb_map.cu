@@ -333,6 +333,7 @@ __device__ __forceinline__ void quad_store_tri(QuadStore& Q, int slot, int tri, 
 //  (Round 1 stored int64 set-ups of every triangle per warp and ran stage C on half-empty warps: 15 of 32 lanes active.)
 template <int kMinBlocks>
 __global__ void __launch_bounds__(kRenderThreads, kMinBlocks) k_render_scatter(KParams kp, SurfelPlanes s, const uint32_t* __restrict__ n_dev,
+                                                                               const uint8_t* __restrict__ live,
                                                                                const float* __restrict__ Mtab, float conf_thr, int t_thr,
                                                                                int emit_old, int emit_new, int lequal, RenderTargets rt) {
   __shared__ QuadStore Q;
@@ -349,9 +350,11 @@ __global__ void __launch_bounds__(kRenderThreads, kMinBlocks) k_render_scatter(K
   float4 p0, p1, p2;
   bool is_old = false, is_new = false;
   if (alive) {
+    // the liveness byte is loaded together with the first two lanes: gating the lanes on it costs an L2 round trip
+    const bool lv = live[k] != 0;
     p2 = __ldg(s.p2 + k);
     p1 = __ldg(s.p1 + k);
-    alive = !kp.use_stability || p1.w > conf_thr;  // .geom:87 (cheap test first)
+    alive = lv && (!kp.use_stability || p1.w > conf_thr);  // .geom:87 (cheap test first)
   }
   if (alive) {
     int creation = (int)p2.w, ts = (int)__float_as_uint(p2.x);
@@ -599,16 +602,17 @@ __global__ void __launch_bounds__(kRenderThreads, kMinBlocks) k_render_scatter(K
   }
 }
 
-void launch_render_scatter(const Launch& L, const KParams& kp, SurfelPlanes s, const uint32_t* n_dev, uint32_t n_upper,
-                           const float* M, float conf_thr, int t_thr, int emit_old, int emit_new, int lequal,
-                           RenderTargets t) {
+void launch_render_scatter(const Launch& L, const KParams& kp, SurfelPlanes s, const uint32_t* n_dev, const uint8_t* live,
+                           uint32_t n_upper, const float* M, float conf_thr, int t_thr, int emit_old, int emit_new,
+                           int lequal, RenderTargets t) {
   if (n_upper == 0) return;
   {
     ScopedKernel sk(L, K_RENDER_SCATTER);
     const unsigned grid = (n_upper + kRenderThreads - 1) / kRenderThreads;
     // 4 resident blocks per SM (64 registers, 46.6 KB shared memory): the kernel is bound by instruction issue and
     // dependent L2 round trips, so occupancy is held at the cost of some spills (microbench.py times the launch)
-    k_render_scatter<4><<<grid, kRenderThreads, 0, L.stream>>>(kp, s, n_dev, M, conf_thr, t_thr, emit_old, emit_new, lequal, t);
+    k_render_scatter<4><<<grid, kRenderThreads, 0, L.stream>>>(kp, s, n_dev, live, M, conf_thr, t_thr, emit_old, emit_new,
+                                                               lequal, t);
   }
 }
 
@@ -718,11 +722,13 @@ void launch_render_resolve(const Launch& L, const KParams& kp, SurfelPlanes s, c
 // K6a: gen_indexmap.vert:62-81 -- nearest visible surfel per data pixel
 // ------------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(kThreads) k_index_scatter(KParams kp, SurfelPlanes s, const uint32_t* __restrict__ n_dev,
-                                                           const float* __restrict__ Mtab,
+                                                           const uint8_t* __restrict__ live, const float* __restrict__ Mtab,
                                                            unsigned long long* __restrict__ keys) {
   uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= *n_dev) return;
+  const bool lv = live[k] != 0;  // (loaded with the lanes, as in k_render_scatter)
   float4 p0 = __ldg(s.p0 + k), p1 = __ldg(s.p1 + k), p2 = __ldg(s.p2 + k);
+  if (!lv) return;
   float M[16];
   load_mat(Mtab, pose_index(p2.w), M);
   V3 v = xform_point(M, mk3(p0.x, p0.y, p0.z));
@@ -741,12 +747,12 @@ __global__ void __launch_bounds__(kThreads) k_index_scatter(KParams kp, SurfelPl
   if (key < keys[pix]) atomicMin(keys + pix, key);
 }
 
-void launch_index_scatter(const Launch& L, const KParams& kp, SurfelPlanes s, const uint32_t* n_dev, uint32_t n_upper,
-                          const float* M, unsigned long long* keys) {
+void launch_index_scatter(const Launch& L, const KParams& kp, SurfelPlanes s, const uint32_t* n_dev, const uint8_t* live,
+                          uint32_t n_upper, const float* M, unsigned long long* keys) {
   if (n_upper == 0) return;
   {
     ScopedKernel sk(L, K_INDEX_SCATTER);
-    k_index_scatter<<<(n_upper + kThreads - 1) / kThreads, kThreads, 0, L.stream>>>(kp, s, n_dev, M, keys);
+    k_index_scatter<<<(n_upper + kThreads - 1) / kThreads, kThreads, 0, L.stream>>>(kp, s, n_dev, live, M, keys);
   }
 }
 
@@ -916,17 +922,40 @@ struct UpdateArgs {
   float submap_extent;
 };
 
+__device__ __forceinline__ bool same_bits(float4 a, float4 b) {
+  return __float_as_uint(a.x) == __float_as_uint(b.x) && __float_as_uint(a.y) == __float_as_uint(b.y) &&
+         __float_as_uint(a.z) == __float_as_uint(b.z) && __float_as_uint(a.w) == __float_as_uint(b.w);
+}
+
+// kLazy = false (dense): the updated records go to tmp with a keep byte each, and k_compact moves the kept ones back.
+// kLazy = true (in place): a lane is stored back into src only if its bits changed, a surfel that is not kept is marked
+// dead in `live`, and nothing moves: counts[1] = the physical end (k_gen_compact appends behind it and sums the live
+// count from the group totals). Dead slots are skipped in both modes, so a dense pass also compacts the map.
+template <bool kLazy>
 __global__ void __launch_bounds__(kThreads) k_update_surfels(KParams kp, SurfelPlanes src, SurfelPlanes tmp,
-                                                            const uint32_t* __restrict__ n_dev, UpdateArgs ua,
+                                                            const uint32_t* n_dev, UpdateArgs ua,
                                                             FrameDev f, uint8_t* __restrict__ integrated,
-                                                            uint8_t* __restrict__ keep,
+                                                            uint8_t* __restrict__ live, uint8_t* __restrict__ keep,
                                                             uint32_t* __restrict__ block_counts,
-                                                            uint32_t* __restrict__ group_counts) {
+                                                            uint32_t* __restrict__ group_counts, uint32_t* counts) {
   uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  const uint32_t n = *n_dev;
+  if (kLazy && k == 0) counts[1] = n;
   bool kept = false;
-  if (k < *n_dev) {
+  bool lv = false;
+  // in place, the lanes are written by this kernel: plain loads, not the read-only path. The liveness byte is loaded
+  // together with them (gating the lane loads on it would cost an L2 round trip per wave).
+  float4 p0, p1, p2, p3 = make_float4(0.f, 0.f, 0.f, 0.f);
+  if (k < n) {
+    lv = live[k] != 0;
+    if (kLazy) {
+      p0 = src.p0[k]; p1 = src.p1[k]; p2 = src.p2[k];
+    } else {
+      p0 = __ldg(src.p0 + k); p1 = __ldg(src.p1 + k); p2 = __ldg(src.p2 + k); p3 = __ldg(src.p3 + k);
+    }
+  }
+  if (lv) {
     const int W = kp.W, H = kp.H;
-    float4 p0 = __ldg(src.p0 + k), p1 = __ldg(src.p1 + k), p2 = __ldg(src.p2 + k), p3 = __ldg(src.p3 + k);
     const int timestamp = ua.timestamp;
     int s_ts = (int)__float_as_uint(p2.x);
     int surfel_age = timestamp - s_ts;
@@ -941,7 +970,9 @@ __global__ void __launch_bounds__(kThreads) k_update_surfels(KParams kp, SurfelP
     float old_radius = p0.w, old_conf = p1.w, old_weight = p2.z;
     bool valid_out = true;
     if (old_conf < kp.confidence_threshold && kp.use_stability) valid_out = surfel_age < kp.unstable_age;
-    float4 o0 = p0, o1 = p1, o2 = p2, o3 = p3;
+    float4 o0 = p0, o1 = p1, o2 = p2;
+    bool avg_prob_set = false;  // o3 = p3 with w = avg_prob
+    float avg_prob = 0.0f;
     o2.y = pack_rgb(0.3f, 0.3f, 0.3f);
     V3 vertex = xform_point(INV, old_position);
     V3 normal = normalize3(xform_dir(INV, old_normal));
@@ -962,6 +993,7 @@ __global__ void __launch_bounds__(kThreads) k_update_surfels(KParams kp, SurfelP
     size_t dpix = 0;
     bool mark_integrated = false;
     if (valid && inside && visible) {
+      if (kLazy) p3 = src.p3[k];  // the only branch that reads or changes the semantic lane
       float4 St = data_tex(f.semantic, W, H, ix, iy);
       float4 Rt = data_tex(ua.radius_map, W, H, ix, iy);
       float data_label = St.x * 255.0f, data_prob = St.w;
@@ -1013,12 +1045,11 @@ __global__ void __launch_bounds__(kThreads) k_update_surfels(KParams kp, SurfelP
           }
           V3 avg_position = add3(scale3(w1, old_position), scale3(w2, v_global));
           V3 avg_normal = slerp(old_normal, n_global, w1);
-          float avg_prob;
           if (label_diff)
             avg_prob = w1 * model_prob + w2 * (1.0f - data_prob);
           else
             avg_prob = w1 * model_prob + w2 * data_prob;
-          o3.w = avg_prob;
+          avg_prob_set = true;
           if (kp.averaging_scheme == 1) {
             avg_position = add3(old_position, scale3(w2 * distance, old_normal));
             avg_normal = slerp(old_normal, n_global, w1);
@@ -1051,12 +1082,22 @@ __global__ void __launch_bounds__(kThreads) k_update_surfels(KParams kp, SurfelP
     if (o1.w < kp.log_unstable && kp.use_stability) valid_out = false;
     if (valid_out && mark_integrated) integrated[dpix] = 1;
     kept = valid_out && submap_keep(ua.poses, o0, o2, ua.submap_center, ua.submap_extent);
-    tmp.p0[k] = o0;
-    tmp.p1[k] = o1;
-    tmp.p2[k] = o2;
-    tmp.p3[k] = o3;
-    keep[k] = kept ? 1 : 0;
+    const float4 o3 = avg_prob_set ? make_float4(p3.x, p3.y, p3.z, avg_prob) : p3;
+    if (!kLazy) {
+      tmp.p0[k] = o0;
+      tmp.p1[k] = o1;
+      tmp.p2[k] = o2;
+      tmp.p3[k] = o3;
+    } else if (!kept) {
+      live[k] = 0;
+    } else {  // bits, not values: -0.0, NaN payloads and confidences above 20 are stored exactly as the dense pass does
+      if (!same_bits(o0, p0)) src.p0[k] = o0;
+      if (!same_bits(o1, p1)) src.p1[k] = o1;
+      if (!same_bits(o2, p2)) src.p2[k] = o2;
+      if (avg_prob_set && __float_as_uint(avg_prob) != __float_as_uint(p3.w)) src.p3[k] = o3;
+    }
   }
+  if (!kLazy && k < n) keep[k] = kept ? 1 : 0;
   // (group totals are cleared by the per-pixel prologue of the map update)
   publish_block_count(kept, block_counts, group_counts);
 }
@@ -1065,8 +1106,9 @@ __global__ void __launch_bounds__(kThreads) k_update_surfels(KParams kp, SurfelP
 __global__ void __launch_bounds__(kThreads) k_gen_compact(KParams kp, FrameDev f, const float4* __restrict__ radius_map,
                                                          const uint8_t* __restrict__ integrated,
                                                          const float* __restrict__ poses, int timestamp, float2 center,
-                                                         float extent, SurfelPlanes dst, Lookback lb, uint32_t cap,
-                                                         uint32_t* __restrict__ counts) {
+                                                         float extent, SurfelPlanes dst, uint8_t* __restrict__ live,
+                                                         const uint32_t* __restrict__ lazy_groups, Lookback lb,
+                                                         uint32_t cap, uint32_t* __restrict__ counts) {
   const uint32_t vb = block_ticket(lb);
   int t = (int)(vb * blockDim.x + threadIdx.x);
   bool kept = false;
@@ -1111,18 +1153,32 @@ __global__ void __launch_bounds__(kThreads) k_gen_compact(KParams kp, FrameDev f
       dst.p1[d] = o1;
       dst.p2[d] = o2;
       dst.p3[d] = o3;
+      live[d] = 1;
+    }
+  }
+  if (vb == gridDim.x - 1 && lazy_groups && threadIdx.x < 32) {
+    // after an in-place update (complete: stream order), which compacted nothing: the surfels it kept are the sum of the
+    // group totals it published, and the rest of the slots below counts[1] are dead
+    uint32_t v = 0;
+    for (int g = threadIdx.x; g < kGroupCounts; g += 32) v += lazy_groups[g];
+    v = __reduce_add_sync(0xffffffffu, v);
+    if (threadIdx.x == 0) {
+      counts[2] = v;
+      counts[5] = base - v;
     }
   }
   if (vb == gridDim.x - 1 && threadIdx.x == 0) {
     uint32_t total = base + excl + block_count;
-    counts[0] = total < cap ? total : cap;  // new size of the map
+    counts[0] = total < cap ? total : cap;  // new physical end of the map
     counts[3] = excl + block_count;         // kept new surfels
     *lb.ticket = 0;
   }
 }
 
-// extract_surfels.vert:44-62: flags of the surfels inside one submap tile
+// extract_surfels.vert:44-62: flags of the live surfels inside one submap tile; with poses == nullptr, of every live
+// surfel (the compaction of a map with dead slots)
 __global__ void __launch_bounds__(kThreads) k_extract_flags(SurfelPlanes s, const uint32_t* __restrict__ n_dev,
+                                                           const uint8_t* __restrict__ live,
                                                            const float* __restrict__ poses, float2 center, float extent,
                                                            uint8_t* __restrict__ keep,
                                                            uint32_t* __restrict__ block_counts,
@@ -1130,11 +1186,16 @@ __global__ void __launch_bounds__(kThreads) k_extract_flags(SurfelPlanes s, cons
   uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
   bool kept = false;
   if (k < *n_dev) {
-    float4 p0 = __ldg(s.p0 + k), p2 = __ldg(s.p2 + k);
-    float M[16];
-    load_mat(poses, pose_index(p2.w), M);
-    V3 w = xform_point(M, mk3(p0.x, p0.y, p0.z));
-    kept = !(fabsf(w.x - center.x) > extent || fabsf(w.y - center.y) > extent);
+    if (live[k]) {
+      kept = true;
+      if (poses) {
+        float4 p0 = __ldg(s.p0 + k), p2 = __ldg(s.p2 + k);
+        float M[16];
+        load_mat(poses, pose_index(p2.w), M);
+        V3 w = xform_point(M, mk3(p0.x, p0.y, p0.z));
+        kept = !(fabsf(w.x - center.x) > extent || fabsf(w.y - center.y) > extent);
+      }
+    }
     keep[k] = kept ? 1 : 0;
   }
   publish_block_count(kept, block_counts, group_counts);
@@ -1145,10 +1206,12 @@ __global__ void __launch_bounds__(kThreads) k_extract_flags(SurfelPlanes s, cons
 // (<= 63), summed by one warp. The kept item of relative rank rel goes to dst[base + rel] iff rel < rel_cap and
 // base + rel < cap (transform feedback drops what does not fit), with base = *base_dev (0 if null; base <= cap).
 // The last block publishes out[0] = base + number written (the end of the written range), out[1] = number kept.
+// dst_live (null for the tile pool): the liveness bytes of the destination slots, set for every slot written.
 __global__ void __launch_bounds__(kThreads) k_compact(SurfelPlanes src, const uint8_t* __restrict__ keep,
                                                      const uint32_t* __restrict__ block_counts,
                                                      const uint32_t* __restrict__ group_counts,
                                                      const uint32_t* __restrict__ n_dev, SurfelPlanes dst,
+                                                     uint8_t* __restrict__ dst_live,
                                                      const uint32_t* __restrict__ base_dev, uint32_t cap, uint32_t rel_cap,
                                                      uint32_t* __restrict__ out) {
   __shared__ uint32_t warp_cnt[kThreads / 32];
@@ -1193,63 +1256,83 @@ __global__ void __launch_bounds__(kThreads) k_compact(SurfelPlanes src, const ui
   dst.p1[d] = src.p1[k];
   dst.p2[d] = src.p2[k];
   dst.p3[d] = src.p3[k];
+  if (dst_live) dst_live[d] = 1;
 }
 
 void launch_compact(const Launch& L, SurfelPlanes src, const uint8_t* keep, const uint32_t* block_counts,
                     const uint32_t* group_counts, const uint32_t* n_dev, uint32_t n_upper, SurfelPlanes dst,
-                    const uint32_t* base_dev, uint32_t cap, uint32_t rel_cap, uint32_t* out) {
+                    uint8_t* dst_live, const uint32_t* base_dev, uint32_t cap, uint32_t rel_cap, uint32_t* out) {
   uint32_t blocks = (n_upper + kThreads - 1) / kThreads;
   if (blocks == 0) blocks = 1;
   {
     ScopedKernel sk(L, K_COMPACT_SCATTER);
-    k_compact<<<blocks, kThreads, 0, L.stream>>>(src, keep, block_counts, group_counts, n_dev, dst, base_dev, cap, rel_cap,
-                                                 out);
+    k_compact<<<blocks, kThreads, 0, L.stream>>>(src, keep, block_counts, group_counts, n_dev, dst, dst_live, base_dev, cap,
+                                                 rel_cap, out);
   }
+}
+
+void launch_compact_live(const Launch& L, SurfelPlanes src, const uint32_t* n_dev, uint32_t n_upper, uint8_t* live,
+                         uint8_t* keep, uint32_t* block_counts, uint32_t* group_counts, SurfelPlanes dst, uint32_t* out) {
+  if (n_upper > 0) {
+    ScopedKernel sk(L, K_EXTRACT_FLAGS);
+    k_extract_flags<<<(n_upper + kThreads - 1) / kThreads, kThreads, 0, L.stream>>>(src, n_dev, live, nullptr,
+                                                                                 make_float2(0.f, 0.f), 0.f, keep,
+                                                                                 block_counts, group_counts);
+  }
+  // (k_extract_flags has consumed the liveness bytes of the source slots before any is set for a destination slot)
+  launch_compact(L, src, keep, block_counts, group_counts, n_dev, n_upper, dst, live, nullptr, kMaxSurfels, kMaxSurfels,
+                 out);
 }
 
 // ---- submap tile cache in HBM: a leaving tile is compacted straight into a device-resident pool (the reference
 // downloads it to host RAM, SurfelMap.cpp:708-742). Slot s of the pool starts where slot s - 1 ends (slot 0 at 0);
 // rec[s] = {end of slot s in the pool, surfels of the tile}.
-void launch_extract_to_pool(const Launch& L, SurfelPlanes map, const uint32_t* n_dev, uint32_t n_upper, const float* poses,
-                            float2 center, float extent, uint8_t* keep, uint32_t* block_counts, uint32_t* group_counts,
-                            SurfelPlanes pool, uint32_t pool_cap, uint2* rec, uint32_t slot, uint32_t tile_cap) {
+void launch_extract_to_pool(const Launch& L, SurfelPlanes map, const uint32_t* n_dev, const uint8_t* live, uint32_t n_upper,
+                            const float* poses, float2 center, float extent, uint8_t* keep, uint32_t* block_counts,
+                            uint32_t* group_counts, SurfelPlanes pool, uint32_t pool_cap, uint2* rec, uint32_t slot,
+                            uint32_t tile_cap) {
   if (n_upper > 0) {
     ScopedKernel sk(L, K_EXTRACT_FLAGS);
-    k_extract_flags<<<(n_upper + kThreads - 1) / kThreads, kThreads, 0, L.stream>>>(map, n_dev, poses, center, extent, keep,
-                                                                                 block_counts, group_counts);
+    k_extract_flags<<<(n_upper + kThreads - 1) / kThreads, kThreads, 0, L.stream>>>(map, n_dev, live, poses, center, extent,
+                                                                                 keep, block_counts, group_counts);
   }
-  launch_compact(L, map, keep, block_counts, group_counts, n_dev, n_upper, pool, slot ? &rec[slot - 1].x : nullptr,
+  launch_compact(L, map, keep, block_counts, group_counts, n_dev, n_upper, pool, nullptr, slot ? &rec[slot - 1].x : nullptr,
                  pool_cap, tile_cap, &rec[slot].x);
 }
 
-void launch_update_surfels(const Launch& L, const KParams& kp, SurfelPlanes src, SurfelPlanes tmp, const uint32_t* n_dev,
-                           uint32_t n_upper, const Mat4& pose, const Mat4& inv_pose, const Mat4* pose_dev,
-                           const Mat4* inv_pose_dev, const float* poses,
+void launch_update_surfels(const Launch& L, const KParams& kp, bool lazy, SurfelPlanes src, SurfelPlanes tmp,
+                           uint32_t* counts, uint32_t n_upper, const Mat4& pose, const Mat4& inv_pose,
+                           const Mat4* pose_dev, const Mat4* inv_pose_dev, const float* poses,
                            const float* poses_inv, const unsigned long long* index_keys, const float4* radius_map,
                            FrameDev frame, int timestamp, float2 submap_center, float submap_extent,
-                           uint8_t* integrated, uint8_t* keep, uint32_t* block_counts, uint32_t* group_counts) {
+                           uint8_t* integrated, uint8_t* live, uint8_t* keep, uint32_t* block_counts,
+                           uint32_t* group_counts) {
   if (n_upper == 0) return;
   UpdateArgs ua{pose, inv_pose, pose_dev, inv_pose_dev, poses, poses_inv, index_keys, radius_map, timestamp,
                 submap_center, submap_extent};
+  const unsigned grid = (n_upper + kThreads - 1) / kThreads;
   {
     ScopedKernel sk(L, K_UPDATE_SURFELS);
-    k_update_surfels<<<(n_upper + kThreads - 1) / kThreads, kThreads, 0, L.stream>>>(kp, src, tmp, n_dev, ua, frame,
-                                                                                  integrated, keep, block_counts,
-                                                                                  group_counts);
+    if (lazy)
+      k_update_surfels<true><<<grid, kThreads, 0, L.stream>>>(kp, src, tmp, counts, ua, frame, integrated, live, keep,
+                                                             block_counts, group_counts, counts);
+    else
+      k_update_surfels<false><<<grid, kThreads, 0, L.stream>>>(kp, src, tmp, counts, ua, frame, integrated, live, keep,
+                                                              block_counts, group_counts, counts);
   }
 }
 
 void launch_gen_compact(const Launch& L, const KParams& kp, FrameDev frame, const float4* radius_map,
                         const uint8_t* integrated, const float* poses, int timestamp, float2 submap_center,
-                        float submap_extent, SurfelPlanes map, unsigned long long* desc, uint32_t* ticket, uint32_t gen,
-                        uint32_t cap, uint32_t* counts) {
+                        float submap_extent, SurfelPlanes map, uint8_t* live, const uint32_t* lazy_groups,
+                        unsigned long long* desc, uint32_t* ticket, uint32_t gen, uint32_t cap, uint32_t* counts) {
   int P = kp.W * kp.H;
   Lookback lb{desc, ticket, gen};
   {
     ScopedKernel sk(L, K_GEN_SURFELS);
     k_gen_compact<<<(P + kThreads - 1) / kThreads, kThreads, 0, L.stream>>>(kp, frame, radius_map, integrated, poses,
                                                                            timestamp, submap_center, submap_extent, map,
-                                                                           lb, cap, counts);
+                                                                           live, lazy_groups, lb, cap, counts);
   }
 }
 
