@@ -121,6 +121,9 @@ struct sb_ctx {
   uint32_t n_upper = 0;  // upper bound used for grid sizing while the exact count is still in flight
   uint32_t n_updated = 0, n_new = 0;
   uint32_t map_timestamp = 0;
+  // one past the largest pose-table entry a surfel of the map or of a cached tile can refer to (creation timestamp,
+  // clamped as pose_index() does): while it is <= map_timestamp, no surfel reads the entry the scan's pose goes into
+  uint32_t pose_ref_end = 0;
   int32_t origin_i = 0, origin_j = 0;
   std::vector<std::pair<int32_t, int32_t>> extraction;
   std::map<std::pair<int32_t, int32_t>, DevTile> tiles;
@@ -274,7 +277,7 @@ int reset_state(sb_ctx* c) {
   // SurfelMap::reset (SurfelMap.cpp:473-482) + the SurfelMapping members set up in its constructor
   c->map_version += 1;
   c->n_host = 0; c->n_holes = 0; c->lazy_update = false;
-  c->n_updated = 0; c->n_new = 0; c->map_timestamp = 0;
+  c->n_updated = 0; c->n_new = 0; c->map_timestamp = 0; c->pose_ref_end = 0;
   c->origin_i = c->origin_j = 0;
   c->extraction.clear();
   c->tiles.clear();
@@ -484,7 +487,7 @@ int render_full(sb_ctx* c, const float* pose_old, const float* pose_new, float c
 
 // which: 1 = active (new surfels into newMapFrame), 0 = inactive (old surfels into oldMapFrame); Q4: semantic map kept
 int render_single(sb_ctx* c, const float* pose, float conf_thr, int which, const Mat4* inv_dev = nullptr,
-                  bool table_ready = false, sb_frame* copy_to = nullptr) {
+                  bool table_ready = false, sb_frame* copy_to = nullptr, const IndexFuse* index = nullptr) {
   frame_written(c, which ? c->f_new : c->f_old);
   if (copy_to) frame_written(c, copy_to);
   const KParams& kp = c->kp;
@@ -496,7 +499,7 @@ int render_single(sb_ctx* c, const float* pose, float conf_thr, int which, const
   unsigned long long* key = which ? c->key_new : c->key_old;
   RenderTargets t{which ? nullptr : key, which ? key : nullptr, nullptr};
   launch_render_scatter(L, kp, c->A, c->res->counts, c->live, n_grid(c), c->Mtab_old, conf_thr, t_threshold(c), which ? 0 : 1,
-                        which ? 1 : 0, 0, t);
+                        which ? 1 : 0, 0, t, index);
   // copy_to: lastModelFrame_->copy(*map_->newMapFrame()), SurfelMapping.cpp:407 (the semantic image is the stale one, Q4),
   // written by the same resolve pass
   launch_render_resolve(L, kp, c->A, c->Mtab_old, c->Mtab_old, t, c->f_old->d, c->f_new->d, null_frame(), null_frame(),
@@ -791,8 +794,9 @@ int update_active_submaps(sb_ctx* c, const float* pose) {  // SurfelMap.cpp:744-
 
 // pose_dev / inv_dev != nullptr: pipeline mode -- the pose (and its pose-table entry) already lives on the device,
 // nothing is read back here; the caller finishes with map_update_finish() after its end-of-scan synchronisation.
+// index_fused: the post-ICP render of this scan has written the index keys unless the track-loss recovery ran (IndexFuse)
 int map_update(sb_ctx* c, const float* pose, const sb_frame* frame, const Mat4* pose_dev = nullptr,
-               const Mat4* inv_dev = nullptr, bool table_ready = false) {
+               const Mat4* inv_dev = nullptr, bool table_ready = false, bool index_fused = false) {
   c->map_version += 1;
   const KParams& kp = c->kp;
   Launch L = L_(c);
@@ -815,7 +819,10 @@ int map_update(sb_ctx* c, const float* pose, const sb_frame* frame, const Mat4* 
   // when the frame is the one it produced
   if (!(c->prepped_for_update && frame == c->cur)) launch_radius(L, kp, frame->d, c->radius_map, c->key_index, c->integrated, c->group_counts);
   c->prepped_for_update = false;
-  launch_index_scatter(L, kp, c->A, c->res->counts, c->live, n_grid(c), c->Mtab_old, c->key_index);
+  // K6a: nearest visible surfel per data pixel. After a fused post-ICP render only a scan with track-loss recovery needs
+  // the pass (P_cur then differs from the render's pose); the launch is gated on that flag on the device.
+  launch_index_scatter(L, kp, c->A, c->res->counts, c->live, n_grid(c), c->Mtab_old, c->key_index,
+                       index_fused ? &c->res->pose.fallback : nullptr);
   // K6c + K6e predicate
   float2 ctr = submap_center(c, c->origin_i, c->origin_j);
   float extent = 2.0f * c->p.submap_dimension * c->p.submap_extent + c->p.submap_extent;  // :674
@@ -848,6 +855,8 @@ int map_update(sb_ctx* c, const float* pose, const sb_frame* frame, const Mat4* 
                      c->res->counts);
   uint64_t up = (uint64_t)n_grid(c) + Pd;  // the map can grow by at most one surfel per pixel
   c->n_upper = up > kMaxSurfels ? kMaxSurfels : (uint32_t)up;
+  const uint32_t entry = c->map_timestamp < kMaxPoses ? c->map_timestamp : kMaxPoses - 1;  // of the new surfels
+  if (entry + 1 > c->pose_ref_end) c->pose_ref_end = entry + 1;
   if (deferred) {
     c->map_timestamp += 1;
     return SB_OK;
@@ -965,10 +974,12 @@ int render_composed_internal(sb_ctx* c, const float* pose_old, const float* pose
 // rendering of the active map at the new pose. Returns with *tables_ready = true when GN_POST has also written the pose
 // table entry of this scan and the table inv(P_cur) * poses[t] (Mtab_old) for the map update / model rendering.
 // With a host all-reduce callback (sb_comm_set_callback) the minimisations are driven from the host instead.
-int update_pose_enqueue(sb_ctx* c, bool* tables_ready) {
+// *index_fused = true: the render at the new pose has also written the map update's index keys (IndexFuse).
+int update_pose_enqueue(sb_ctx* c, bool* tables_ready, bool* index_fused) {
   const sb_params& p = c->p;
   const bool sem = c->cur_has_semantics;
   *tables_ready = false;
+  *index_fused = false;
   int r;
   Launch L = L_(c);
   const uint32_t np = pose_table_count(c);
@@ -998,8 +1009,19 @@ int update_pose_enqueue(sb_ctx* c, bool* tables_ready) {
       cudaGetLastError();
       return fail(c, SB_ERR_CUDA, "cooperative launch of the Gauss-Newton kernel failed");
     }
-    // :405-413: render_active at the new pose (its product table is ready), copied into lastModelFrame_
-    if ((r = render_single(c, nullptr, conf_threshold(c), 1, &c->res->pose.invP_active, true, c->last_model))) return r;
+    // :405-413: render_active at the new pose (its product table is ready), copied into lastModelFrame_.
+    // It also writes the index keys of the map update (K6a) when that pass would see what it sees: without track-loss
+    // recovery P_cur is bit for bit P_active (the same fp64 product, rounded once), GN_POST's table inv(P_cur) * poses[t]
+    // equals this one except at entry t_map, which it sets to P_cur and no surfel refers to while pose_ref_end <=
+    // t_map, and nothing writes the map before the update unless the loop-closure step runs in between.
+    const bool fuse = !c->close_loops && c->pose_ref_end <= c->map_timestamp;
+    // (fov_up, fov, min_depth, max_depth of the data image, then the same four of the model image: bitwise equal?)
+    const int same_projection = memcmp(&c->kp.fov_up, &c->kp.m_fov_up, 4 * sizeof(float)) == 0 ? 1 : 0;
+    const IndexFuse ix{c->key_index, &c->res->pose.fallback, same_projection};
+    if ((r = render_single(c, nullptr, conf_threshold(c), 1, &c->res->pose.invP_active, true, c->last_model,
+                           fuse ? &ix : nullptr)))
+      return r;
+    *index_fused = fuse;
     // :414-449: statistics pass at identity, track-loss recovery, pose chaining, pose-table entry, table for the update
     GnJob post;
     memset(&post, 0, sizeof(post));
@@ -1534,6 +1556,11 @@ int sb_map_upload(sb_ctx* c, const sb_surfel* src, uint32_t n, uint32_t timestam
     launch_aos_to_soa(L_(c), reinterpret_cast<const sb_surfel*>(c->T.p0), c->A, 0, n);
     SB_CUDA(c, cudaMemsetAsync(c->live, 1, n, c->stream));
   }
+  for (uint32_t i = 0; i < n; ++i) {  // the pose-table entry of each surfel, as pose_index() reads it from the count field
+    const float t = src[i].count;
+    const uint32_t e = !(t >= 1.0f) ? 0u : t >= (float)(kMaxPoses - 1) ? kMaxPoses - 1 : (uint32_t)t;
+    if (e + 1 > c->pose_ref_end) c->pose_ref_end = e + 1;
+  }
   c->n_host = n;
   c->n_holes = 0;  // (overwritten: nothing to compact)
   c->n_upper = n;
@@ -1595,10 +1622,10 @@ int sb_process_scan(sb_ctx* c, const float* pts4, const float* labels, const flo
   cast_f(c->currentPose_new, Pnew);
   if ((r = render_full(c, Pold, Pnew, ct, c->last_model))) return r;
   const bool had_icp = c->timestamp > 0;
-  bool tables_ready = false;
+  bool tables_ready = false, index_fused = false;
   bool loop_ran = false;
   if (had_icp) {
-    if ((r = update_pose_enqueue(c, &tables_ready))) return r;
+    if ((r = update_pose_enqueue(c, &tables_ready, &index_fused))) return r;
     if (c->close_loops) {  // checkLoopClosure(), :196-200; its renders overwrite the product table of the map update
       if ((r = loop_closure_step(c))) return r;
       tables_ready = false;
@@ -1609,7 +1636,8 @@ int sb_process_scan(sb_ctx* c, const float* pts4, const float* labels, const flo
   }
   // updateMap(), :797-804
   const uint32_t t_map = c->map_timestamp;
-  if ((r = map_update(c, nullptr, c->cur, &c->res->pose.P_cur, &c->res->pose.invP_cur, tables_ready))) return r;
+  if ((r = map_update(c, nullptr, c->cur, &c->res->pose.P_cur, &c->res->pose.invP_cur, tables_ready, index_fused)))
+    return r;
   float ct2 = conf_threshold(c);
   if (p.render_after_update) {
     if ((r = render_full(c, nullptr, nullptr, ct2, c->cur_model, &c->res->pose.invP_cur, true))) return r;

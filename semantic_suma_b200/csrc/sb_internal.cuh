@@ -250,17 +250,27 @@ struct RenderTargets {
   unsigned long long* key_new;   // may be null
   unsigned long long* key_comp;  // may be null
 };
+// The map update's index keys (K6a), written by the post-ICP render of the pipeline: that render and the index pass
+// read the same map at the same pose with the same product table whenever the track-loss recovery does not run, so the
+// render computes the keys from the transform, visibility test and centre projection it has already done.
+struct IndexFuse {
+  unsigned long long* keys;  // the index keys, armed this scan
+  const int* fallback;       // PoseDev::fallback of the scan: set -> no keys here, the gated index pass writes them all
+  int same_projection;       // model and data projection parameters are bitwise equal: the render's projection serves
+};
 void launch_pose_products(const Launch& L, const Mat4& A, const Mat4* A_dev, const float* poses, float* out,
                           uint32_t count);
 // Surfel slots [0, counts[0]) of the map; a slot whose liveness byte is 0 holds a surfel removed by an in-place update.
+// index != null: also write the index keys (IndexFuse).
 void launch_render_scatter(const Launch& L, const KParams& kp, SurfelPlanes s, const uint32_t* n_dev, const uint8_t* live,
                            uint32_t n_upper, const float* M, float conf_thr, int t_thr, int emit_old, int emit_new,
-                           int lequal, RenderTargets t);
+                           int lequal, RenderTargets t, const IndexFuse* index = nullptr);
 void launch_render_resolve(const Launch& L, const KParams& kp, SurfelPlanes s, const float* M_old, const float* M_new,
                            RenderTargets t, FrameDev f_old, FrameDev f_new, FrameDev f_comp, FrameDev f_out,
                            FrameDev f_copy, int keep_semantic, int lequal);
+// gate != null: runs only if *gate is set (the repair of a fused scan on which the track-loss recovery ran)
 void launch_index_scatter(const Launch& L, const KParams& kp, SurfelPlanes s, const uint32_t* n_dev, const uint8_t* live,
-                          uint32_t n_upper, const float* M, unsigned long long* keys);
+                          uint32_t n_upper, const float* M, unsigned long long* keys, const int* gate = nullptr);
 void launch_radius(const Launch& L, const KParams& kp, FrameDev frame, float4* radius_map, unsigned long long* index_keys,
                    uint8_t* integrated, uint32_t* group_counts);
 // ordered compaction of a surfel-indexed pass: items flagged in keep[0..n) of src go to dst[base..) in order, base =

@@ -319,6 +319,22 @@ __device__ __forceinline__ void quad_store_tri(QuadStore& Q, int slot, int tri, 
   Q.farea[tri][slot] = t.farea;
 }
 
+// K6a, gen_indexmap.vert:62-81 for one visible surfel k whose centre projects to (x, y, z) under the data image's
+// parameters: its depth key and data pixel, false if it lands on none (k_index_scatter, and k_render_scatter<., true>
+// for the pipeline; both then keep the smaller key with a stale pre-read and atomicMin, as emit_fragment does)
+__device__ __forceinline__ bool index_key(const KParams& kp, float x, float y, float z, uint32_t k,
+                                          unsigned long long& key, size_t& pix) {
+  float fx = floorf(x * (float)kp.W), fy = floorf(y * (float)kp.H);
+  if (!(fx >= 0.0f && fx < (float)kp.W && fy >= 0.0f && fy < (float)kp.H)) return false;
+  float zn = 2.0f * z - 1.0f;
+  if (!(zn >= -1.0f && zn <= 1.0f)) return false;
+  uint32_t d24 = depth24(0.5f * zn + 0.5f);
+  if (d24 >= kDepthClear) return false;
+  pix = (size_t)(int)fy * kp.W + (size_t)(int)fx;
+  key = ((unsigned long long)d24 << 32) | (unsigned long long)k;
+  return true;
+}
+
 // render_surfels.vert:42-54 + .geom:76-122 + rasterisation + depth test for every surfel of the map.
 //  stage A/B (one thread per surfel): confidence / age-class tests on two lanes, then transform, visibility and the
 //    projection of the centre -- about half of the map drops out here;
@@ -331,11 +347,13 @@ __device__ __forceinline__ void quad_store_tri(QuadStore& Q, int slot, int tri, 
 //    "small" quad (box <= 12 x 5 pixels, vertices within 64 pixels) keeps every product below 2^31; the rare larger
 //    quads are rasterised by whole warps with int64 edge functions.
 //  (Round 1 stored int64 set-ups of every triangle per warp and ran stage C on half-empty warps: 15 of 32 lanes active.)
-template <int kMinBlocks>
+// kIndex: the render also writes the map update's index keys (K6a, index_key()) for every live surfel, see IndexFuse.
+template <int kMinBlocks, bool kIndex>
 __global__ void __launch_bounds__(kRenderThreads, kMinBlocks) k_render_scatter(KParams kp, SurfelPlanes s, const uint32_t* __restrict__ n_dev,
                                                                                const uint8_t* __restrict__ live,
                                                                                const float* __restrict__ Mtab, float conf_thr, int t_thr,
-                                                                               int emit_old, int emit_new, int lequal, RenderTargets rt) {
+                                                                               int emit_old, int emit_new, int lequal, RenderTargets rt,
+                                                                               IndexFuse ix) {
   __shared__ QuadStore Q;
   __shared__ float c_f[8][kRenderThreads];
   __shared__ uint32_t c_flags[kRenderThreads];
@@ -348,12 +366,16 @@ __global__ void __launch_bounds__(kRenderThreads, kMinBlocks) k_render_scatter(K
   const uint32_t k = blockIdx.x * blockDim.x + tid;
   bool alive = k < *n_dev;
   float4 p0, p1, p2;
-  bool is_old = false, is_new = false;
+  bool is_old = false, is_new = false, indexed = false;
   if (alive) {
     // the liveness byte is loaded together with the first two lanes: gating the lanes on it costs an L2 round trip
     const bool lv = live[k] != 0;
     p2 = __ldg(s.p2 + k);
     p1 = __ldg(s.p1 + k);
+    if (kIndex) {  // the index map needs every live surfel: p0 joins the first loads instead of waiting for the tests
+      p0 = __ldg(s.p0 + k);
+      indexed = lv && *ix.fallback == 0;
+    }
     alive = lv && (!kp.use_stability || p1.w > conf_thr);  // .geom:87 (cheap test first)
   }
   if (alive) {
@@ -363,16 +385,23 @@ __global__ void __launch_bounds__(kRenderThreads, kMinBlocks) k_render_scatter(K
     alive = is_old || is_new;
   }
   Cand c;
-  if (alive) {
-    p0 = __ldg(s.p0 + k);
+  if (alive || indexed) {
+    if (!kIndex) p0 = __ldg(s.p0 + k);
     float M[16];
     load_mat(Mtab, pose_index(p2.w), M);
     V3 pp = xform_point(M, mk3(p0.x, p0.y, p0.z));
     V3 nn = xform_dir(M, mk3(p1.x, p1.y, p1.z));
-    bool visible = dot3(nn, divs3(neg3(pp), len3(pp))) > 0.01f;  // .geom:84
+    bool visible = dot3(nn, divs3(neg3(pp), len3(pp))) > 0.01f;  // .geom:84, the same test as gen_indexmap.vert
     float cx, cy, cz;
     project01(pp, kp.m_fov_up, kp.m_fov, kp.m_min_depth, kp.m_max_depth, cx, cy, cz);
-    alive = visible && cx >= 0.0f && cy >= 0.0f && cz >= 0.0f && cx < 1.0f && cy < 1.0f && cz < 1.0f;
+    if (kIndex && indexed && visible) {
+      float x = cx, y = cy, z = cz;
+      if (!ix.same_projection) project01(pp, kp.fov_up, kp.fov, kp.min_depth, kp.max_depth, x, y, z);
+      unsigned long long key;
+      size_t pix;
+      if (index_key(kp, x, y, z, k, key, pix) && key < ix.keys[pix]) atomicMin(ix.keys + pix, key);
+    }
+    alive = alive && visible && cx >= 0.0f && cy >= 0.0f && cz >= 0.0f && cx < 1.0f && cy < 1.0f && cz < 1.0f;
     c.px = pp.x; c.py = pp.y; c.pz = pp.z; c.nx = nn.x; c.ny = nn.y; c.nz = nn.z; c.r = p0.w; c.cx = cx;
   }
   // ---- dense packing of the survivors (their order inside the block is irrelevant: visibility is decided by the keys) ----
@@ -604,15 +633,19 @@ __global__ void __launch_bounds__(kRenderThreads, kMinBlocks) k_render_scatter(K
 
 void launch_render_scatter(const Launch& L, const KParams& kp, SurfelPlanes s, const uint32_t* n_dev, const uint8_t* live,
                            uint32_t n_upper, const float* M, float conf_thr, int t_thr, int emit_old, int emit_new,
-                           int lequal, RenderTargets t) {
+                           int lequal, RenderTargets t, const IndexFuse* index) {
   if (n_upper == 0) return;
   {
     ScopedKernel sk(L, K_RENDER_SCATTER);
     const unsigned grid = (n_upper + kRenderThreads - 1) / kRenderThreads;
     // 4 resident blocks per SM (64 registers, 46.6 KB shared memory): the kernel is bound by instruction issue and
     // dependent L2 round trips, so occupancy is held at the cost of some spills (microbench.py times the launch)
-    k_render_scatter<4><<<grid, kRenderThreads, 0, L.stream>>>(kp, s, n_dev, live, M, conf_thr, t_thr, emit_old, emit_new,
-                                                               lequal, t);
+    if (index)
+      k_render_scatter<4, true><<<grid, kRenderThreads, 0, L.stream>>>(kp, s, n_dev, live, M, conf_thr, t_thr, emit_old,
+                                                                       emit_new, lequal, t, *index);
+    else
+      k_render_scatter<4, false><<<grid, kRenderThreads, 0, L.stream>>>(kp, s, n_dev, live, M, conf_thr, t_thr, emit_old,
+                                                                        emit_new, lequal, t, IndexFuse{});
   }
 }
 
@@ -721,38 +754,40 @@ void launch_render_resolve(const Launch& L, const KParams& kp, SurfelPlanes s, c
 // ------------------------------------------------------------------------------------------------------------
 // K6a: gen_indexmap.vert:62-81 -- nearest visible surfel per data pixel
 // ------------------------------------------------------------------------------------------------------------
+// gate != null: nothing to do unless *gate is set (the track-loss flag of a scan whose post-ICP render was to write the
+// keys, see IndexFuse); the grid is then small and strides over the map.
+constexpr uint32_t kIndexRepairBlocks = 512;
 __global__ void __launch_bounds__(kThreads) k_index_scatter(KParams kp, SurfelPlanes s, const uint32_t* __restrict__ n_dev,
                                                            const uint8_t* __restrict__ live, const float* __restrict__ Mtab,
-                                                           unsigned long long* __restrict__ keys) {
-  uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
-  if (k >= *n_dev) return;
-  const bool lv = live[k] != 0;  // (loaded with the lanes, as in k_render_scatter)
-  float4 p0 = __ldg(s.p0 + k), p1 = __ldg(s.p1 + k), p2 = __ldg(s.p2 + k);
-  if (!lv) return;
-  float M[16];
-  load_mat(Mtab, pose_index(p2.w), M);
-  V3 v = xform_point(M, mk3(p0.x, p0.y, p0.z));
-  V3 n = xform_dir(M, mk3(p1.x, p1.y, p1.z));
-  if (!(dot3(n, divs3(neg3(v), len3(v))) > 0.01f)) return;
-  float x, y, z;
-  project01(v, kp.fov_up, kp.fov, kp.min_depth, kp.max_depth, x, y, z);
-  float fx = floorf(x * (float)kp.W), fy = floorf(y * (float)kp.H);
-  if (!(fx >= 0.0f && fx < (float)kp.W && fy >= 0.0f && fy < (float)kp.H)) return;
-  float zn = 2.0f * z - 1.0f;
-  if (!(zn >= -1.0f && zn <= 1.0f)) return;
-  uint32_t d24 = depth24(0.5f * zn + 0.5f);
-  if (d24 >= kDepthClear) return;
-  size_t pix = (size_t)(int)fy * kp.W + (size_t)(int)fx;
-  unsigned long long key = ((unsigned long long)d24 << 32) | (unsigned long long)k;
-  if (key < keys[pix]) atomicMin(keys + pix, key);
+                                                           unsigned long long* __restrict__ keys, const int* __restrict__ gate) {
+  if (gate && *gate == 0) return;
+  const uint32_t n = *n_dev;
+  for (uint32_t k = blockIdx.x * blockDim.x + threadIdx.x; k < n; k += gridDim.x * blockDim.x) {
+    const bool lv = live[k] != 0;  // (loaded with the lanes, as in k_render_scatter)
+    float4 p0 = __ldg(s.p0 + k), p1 = __ldg(s.p1 + k), p2 = __ldg(s.p2 + k);
+    if (!lv) continue;
+    float M[16];
+    load_mat(Mtab, pose_index(p2.w), M);
+    V3 v = xform_point(M, mk3(p0.x, p0.y, p0.z));
+    V3 nrm = xform_dir(M, mk3(p1.x, p1.y, p1.z));
+    if (!(dot3(nrm, divs3(neg3(v), len3(v))) > 0.01f)) continue;
+    float x, y, z;
+    project01(v, kp.fov_up, kp.fov, kp.min_depth, kp.max_depth, x, y, z);
+    unsigned long long key;
+    size_t pix;
+    if (index_key(kp, x, y, z, k, key, pix) && key < keys[pix]) atomicMin(keys + pix, key);
+  }
 }
 
 void launch_index_scatter(const Launch& L, const KParams& kp, SurfelPlanes s, const uint32_t* n_dev, const uint8_t* live,
-                          uint32_t n_upper, const float* M, unsigned long long* keys) {
+                          uint32_t n_upper, const float* M, unsigned long long* keys, const int* gate) {
   if (n_upper == 0) return;
   {
     ScopedKernel sk(L, K_INDEX_SCATTER);
-    k_index_scatter<<<(n_upper + kThreads - 1) / kThreads, kThreads, 0, L.stream>>>(kp, s, n_dev, live, M, keys);
+    // gated: a grid that costs next to nothing when the gate is clear and still covers the map when it is set
+    const uint32_t blocks = (n_upper + kThreads - 1) / kThreads;
+    const uint32_t grid = gate && blocks > kIndexRepairBlocks ? kIndexRepairBlocks : blocks;
+    k_index_scatter<<<grid, kThreads, 0, L.stream>>>(kp, s, n_dev, live, M, keys, gate);
   }
 }
 
