@@ -71,9 +71,9 @@ void launch_pose_products(const Launch& L, const Mat4& A, const Mat4* A_dev, con
 // ------------------------------------------------------------------------------------------------------------
 // K4 rasteriser
 // ------------------------------------------------------------------------------------------------------------
-struct RVert {
+struct RVert {  // the texture coordinates of quad corner i are (i & 1 ? 1 : -1, i & 2 ? 1 : -1), see corner_tx()
   long long X, Y;
-  float z, tx, ty;
+  float z;
 };
 
 __device__ __forceinline__ long long floor_div256(long long a) { return a >> 8; }  // arithmetic shift = floor
@@ -95,18 +95,18 @@ struct TriSetup {
   long long sxA, sxB, sxC;  // step per pixel in x
   long long syA, syB, syC;  // step per pixel in y
   float farea;
-  float zA, zB, zC, txA, txB, txC, tyA, tyB, tyC;
+  float zA, zB, zC;
   int i0, j0, ni, nj;       // bounding box origin and extent (inclusive), clamped to the image
-  uint32_t ties;            // bit0..2: pixels exactly on edge A/B/C count as inside
+  uint32_t ties;            // bit0..2: pixels exactly on edge A/B/C count as inside, bit3: B and C were swapped
   uint32_t valid;
 };
 
-__device__ __forceinline__ TriSetup tri_prepare(RVert A, RVert B, RVert C, int W, int H) {
-  TriSetup t;
+__device__ __forceinline__ void tri_prepare(RVert A, RVert B, RVert C, int W, int H, TriSetup& t) {
   t.valid = 0;
   long long area = (B.X - A.X) * (C.Y - A.Y) - (B.Y - A.Y) * (C.X - A.X);
-  if (area == 0) return t;
-  if (area < 0) {
+  if (area == 0) return;
+  const bool swapped = area < 0;
+  if (swapped) {
     RVert x = B;
     B = C;
     C = x;
@@ -120,7 +120,7 @@ __device__ __forceinline__ TriSetup tri_prepare(RVert A, RVert B, RVert C, int W
   if (j0 < 0) j0 = 0;
   if (i1 > W - 1) i1 = W - 1;
   if (j1 > H - 1) j1 = H - 1;
-  if (i0 > i1 || j0 > j1) return t;
+  if (i0 > i1 || j0 > j1) return;
   t.farea = (float)area;
   const long long X0 = i0 * 256 + 128, Y0 = j0 * 256 + 128;
   t.eA = edge_fn(B, C, X0, Y0);
@@ -128,13 +128,10 @@ __device__ __forceinline__ TriSetup tri_prepare(RVert A, RVert B, RVert C, int W
   t.eC = edge_fn(A, B, X0, Y0);
   t.sxA = -256 * (C.Y - B.Y); t.sxB = -256 * (A.Y - C.Y); t.sxC = -256 * (B.Y - A.Y);
   t.syA = 256 * (C.X - B.X); t.syB = 256 * (A.X - C.X); t.syC = 256 * (B.X - A.X);
-  t.ties = (edge_tie(B, C) ? 1u : 0u) | (edge_tie(C, A) ? 2u : 0u) | (edge_tie(A, B) ? 4u : 0u);
+  t.ties = (edge_tie(B, C) ? 1u : 0u) | (edge_tie(C, A) ? 2u : 0u) | (edge_tie(A, B) ? 4u : 0u) | (swapped ? 8u : 0u);
   t.zA = A.z; t.zB = B.z; t.zC = C.z;
-  t.txA = A.tx; t.txB = B.tx; t.txC = C.tx;
-  t.tyA = A.ty; t.tyB = B.ty; t.tyC = C.ty;
   t.i0 = (int)i0; t.j0 = (int)j0; t.ni = (int)(i1 - i0); t.nj = (int)(j1 - j0);
   t.valid = 1;
-  return t;
 }
 
 constexpr int kRenderThreads = 256;
@@ -152,32 +149,36 @@ struct Cand {
   uint32_t k, flags;  // flags: bit0 old-class surfel, bit1 new-class surfel, bit2 GL_LEQUAL composed mode
 };
 
-// render_surfels.geom:80-82, 100-118: the four quad corners in window coordinates (1/256 pixel)
-__device__ __forceinline__ void quad_corners(const KParams& kp, const Cand& c, RVert q[4]) {
-  const V3 pp = mk3(c.px, c.py, c.pz), nn = mk3(c.nx, c.ny, c.nz);
+// render_surfels.geom:80-82: the quad's half axes r*u and r*v
+__device__ __forceinline__ void quad_axes(const Cand& c, V3& ru, V3& rv) {
+  const V3 nn = mk3(c.nx, c.ny, c.nz);
   V3 u = normalize3(mk3(nn.y - nn.z, -nn.x, nn.x));
   V3 v = normalize3(cross3(nn, u));
-  V3 ru = scale3(c.r, u), rv = scale3(c.r, v);
-  V3 corner[4];
-  corner[0] = sub3(sub3(pp, ru), rv);
-  corner[1] = sub3(add3(pp, ru), rv);
-  corner[2] = add3(sub3(pp, ru), rv);
-  corner[3] = add3(add3(pp, ru), rv);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    float x, y, z;
-    project01(corner[i], kp.m_fov_up, kp.m_fov, kp.m_min_depth, kp.m_max_depth, x, y, z);
-    if (c.cx - x > 0.5f) x += 1.0f;  // .geom:68
-    if (x - c.cx > 0.5f) x -= 1.0f;  // .geom:69
-    float xw = (0.5f * (2.0f * x - 1.0f) + 0.5f) * (float)kp.Wm;
-    float yw = (0.5f * (2.0f * y - 1.0f) + 0.5f) * (float)kp.Hm;
-    q[i].z = 0.5f * (2.0f * z - 1.0f) + 0.5f;
-    q[i].X = __float2ll_rn(xw * 256.0f);
-    q[i].Y = __float2ll_rn(yw * 256.0f);
-    q[i].tx = (i & 1) ? 1.0f : -1.0f;
-    q[i].ty = (i & 2) ? 1.0f : -1.0f;
-  }
+  ru = scale3(c.r, u);
+  rv = scale3(c.r, v);
 }
+
+// render_surfels.geom:100-118: quad corner i = (pp -/+ ru) -/+ rv in window coordinates (1/256 pixel)
+__device__ __forceinline__ RVert quad_corner(const KParams& kp, const Cand& c, V3 ru, V3 rv, int i) {
+  const V3 pp = mk3(c.px, c.py, c.pz);
+  const V3 h = (i & 1) ? add3(pp, ru) : sub3(pp, ru);
+  const V3 corner = (i & 2) ? add3(h, rv) : sub3(h, rv);
+  float x, y, z;
+  project01(corner, kp.m_fov_up, kp.m_fov, kp.m_min_depth, kp.m_max_depth, x, y, z);
+  if (c.cx - x > 0.5f) x += 1.0f;  // .geom:68
+  if (x - c.cx > 0.5f) x -= 1.0f;  // .geom:69
+  float xw = (0.5f * (2.0f * x - 1.0f) + 0.5f) * (float)kp.Wm;
+  float yw = (0.5f * (2.0f * y - 1.0f) + 0.5f) * (float)kp.Hm;
+  RVert q;
+  q.z = 0.5f * (2.0f * z - 1.0f) + 0.5f;
+  q.X = __float2ll_rn(xw * 256.0f);
+  q.Y = __float2ll_rn(yw * 256.0f);
+  return q;
+}
+
+// texture coordinates of quad corner i (render_surfels.geom:100-118)
+__device__ __forceinline__ float corner_tx(int i) { return (i & 1) ? 1.0f : -1.0f; }
+__device__ __forceinline__ float corner_ty(int i) { return (i & 2) ? 1.0f : -1.0f; }
 
 // fragment stage (render_surfels.frag:19-33) + depth test + key update, shared by both rasterisers
 __device__ __forceinline__ void emit_fragment(float tx, float ty, float z, size_t pix, uint32_t k, uint32_t flags,
@@ -212,90 +213,57 @@ __device__ __forceinline__ void emit_fragment(float tx, float ty, float z, size_
   }
 }
 
-// One triangle of a small quad, everything relative to the quad's first pixel centre (X0, Y0): all magnitudes stay below
-// 2^14 + 2^10, so the int32 edge functions, their steps and the area equal the int64 ones of tri_prepare() bit for bit.
-struct TriSmall {
-  int eA, eB, eC, sxA, sxB, sxC, syA, syB, syC;
-  float farea, zA, zB, zC, txA, txB, txC, tyA, tyB, tyC;
-  uint32_t ties, valid, swapped;
-};
-__device__ __forceinline__ int edge32(int Px, int Py, int Qx, int Qy) {  // edge_fn(P, Q, X0, Y0), P and Q relative to (X0, Y0)
-  return (Qx - Px) * (0 - Py) - (Qy - Py) * (0 - Px);
-}
-__device__ __forceinline__ bool tie32(int Px, int Py, int Qx, int Qy) {
-  int dx = Qx - Px, dy = Qy - Py;
-  return dy > 0 || (dy == 0 && dx > 0);
-}
-__device__ __forceinline__ TriSmall tri_small(const RVert& a, const RVert& b0, const RVert& c0, long long X0, long long Y0) {
-  TriSmall t;
-  t.valid = 0;
-  t.swapped = 0;
-  int Ax = (int)(a.X - X0), Ay = (int)(a.Y - Y0);
-  int Bx = (int)(b0.X - X0), By = (int)(b0.Y - Y0);
-  int Cx = (int)(c0.X - X0), Cy = (int)(c0.Y - Y0);
-  float zB = b0.z, zC = c0.z, txB = b0.tx, txC = c0.tx, tyB = b0.ty, tyC = c0.ty;
-  int area = (Bx - Ax) * (Cy - Ay) - (By - Ay) * (Cx - Ax);
-  if (area == 0) return t;
-  if (area < 0) {  // same orientation fix as tri_prepare(): swap B and C
-    int ti = Bx; Bx = Cx; Cx = ti;
-    ti = By; By = Cy; Cy = ti;
-    float tf = zB; zB = zC; zC = tf;
-    tf = txB; txB = txC; txC = tf;
-    tf = tyB; tyB = tyC; tyC = tf;
-    area = -area;
-    t.swapped = 1;
+// one triangle of a large quad, rasterised by a whole warp: the lanes stride over its bounding-box pixels (int64 edges)
+// (corners tri, tri + 1, tri + 2 of the quad, B and C exchanged if the orientation fix swapped them)
+__device__ __forceinline__ void raster_big_tri(const KParams& kp, const TriSetup& t, int tri, uint32_t k, uint32_t flags,
+                                               const RenderTargets& rt, int lane) {
+  if (!t.valid) return;
+  const int wd = t.ni + 1, total = wd * (t.nj + 1);
+  const bool tieA = t.ties & 1u, tieB = t.ties & 2u, tieC = t.ties & 4u;
+  const int cA = tri, cB = (t.ties & 8u) ? tri + 2 : tri + 1, cC = (t.ties & 8u) ? tri + 1 : tri + 2;
+  const float txA = corner_tx(cA), txB = corner_tx(cB), txC = corner_tx(cC);
+  const float tyA = corner_ty(cA), tyB = corner_ty(cB), tyC = corner_ty(cC);
+  for (int item = lane; item < total; item += 32) {
+    const int dj = item / wd, di = item - dj * wd;
+    const long long wA = t.eA + (long long)di * t.sxA + (long long)dj * t.syA;
+    const long long wB = t.eB + (long long)di * t.sxB + (long long)dj * t.syB;
+    const long long wC = t.eC + (long long)di * t.sxC + (long long)dj * t.syC;
+    const bool in = (wA > 0 || (wA == 0 && tieA)) && (wB > 0 || (wB == 0 && tieB)) && (wC > 0 || (wC == 0 && tieC));
+    if (!in) continue;
+    float fB = (float)wB / t.farea, fC = (float)wC / t.farea;
+    float fA = (1.0f - fB) - fC;
+    float tx = (fA * txA + fB * txB) + fC * txC;
+    float ty = (fA * tyA + fB * tyB) + fC * tyC;
+    float z = (fA * t.zA + fB * t.zB) + fC * t.zC;
+    emit_fragment(tx, ty, z, (size_t)(t.j0 + dj) * kp.Wm + (size_t)(t.i0 + di), k, flags, rt);
   }
-  t.farea = (float)area;
-  t.eA = edge32(Bx, By, Cx, Cy);
-  t.eB = edge32(Cx, Cy, Ax, Ay);
-  t.eC = edge32(Ax, Ay, Bx, By);
-  t.sxA = -256 * (Cy - By); t.sxB = -256 * (Ay - Cy); t.sxC = -256 * (By - Ay);
-  t.syA = 256 * (Cx - Bx); t.syB = 256 * (Ax - Cx); t.syC = 256 * (Bx - Ax);
-  t.ties = (tie32(Bx, By, Cx, Cy) ? 1u : 0u) | (tie32(Cx, Cy, Ax, Ay) ? 2u : 0u) | (tie32(Ax, Ay, Bx, By) ? 4u : 0u);
-  t.zA = a.z; t.zB = zB; t.zC = zC;
-  t.txA = a.tx; t.txB = txB; t.txC = txC;
-  t.tyA = a.ty; t.tyB = tyB; t.tyC = tyC;
-  t.valid = 1;
-  return t;
-}
-__device__ __forceinline__ void tri_small_pixel(const TriSmall& t, int di, int dj, size_t pix, uint32_t k, uint32_t flags,
-                                                const RenderTargets& rt) {
-  const int wA = t.eA + di * t.sxA + dj * t.syA, wB = t.eB + di * t.sxB + dj * t.syB, wC = t.eC + di * t.sxC + dj * t.syC;
-  const bool in = (wA > 0 || (wA == 0 && (t.ties & 1u))) && (wB > 0 || (wB == 0 && (t.ties & 2u))) &&
-                  (wC > 0 || (wC == 0 && (t.ties & 4u)));
-  if (!in) return;
-  float fB = (float)wB / t.farea, fC = (float)wC / t.farea;
-  float fA = (1.0f - fB) - fC;
-  float tx = (fA * t.txA + fB * t.txB) + fC * t.txC;
-  float ty = (fA * t.tyA + fB * t.tyB) + fC * t.tyC;
-  float z = (fA * t.zA + fB * t.zB) + fC * t.zC;
-  emit_fragment(tx, ty, z, pix, k, flags, rt);
 }
 
-// a large quad, rasterised by a whole warp: the lanes stride over the bounding-box pixels of each triangle (int64 edges)
-__device__ __forceinline__ void raster_big(const KParams& kp, const Cand& c, const RenderTargets& rt, int lane) {
-  RVert q[4];
-  quad_corners(kp, c, q);
+// corner i of the quad, held by lanes i, i + 4, ... of the warp
+__device__ __forceinline__ RVert shfl_corner(const RVert& mine, int i) {
+  RVert q;
+  q.X = __shfl_sync(0xffffffffu, mine.X, i);
+  q.Y = __shfl_sync(0xffffffffu, mine.Y, i);
+  q.z = __shfl_sync(0xffffffffu, mine.z, i);
+  return q;
+}
+
+// a large quad (warp-uniform): every lane projects one corner, and each triangle collects its three corners by shuffles,
+// so that no corner array stays live next to a triangle's set-up. The set-up itself goes to `st`, the warp's slot in
+// shared memory, and the pixel loop reads it from there: held in registers next to the fragment evaluation it needed
+// ~76 registers and spilled at the 64 that 4 blocks per SM allow.
+__device__ __forceinline__ void raster_big(const KParams& kp, const Cand& c, const RenderTargets& rt, int lane,
+                                           TriSetup& st) {
+  V3 ru, rv;
+  quad_axes(c, ru, rv);
+  const RVert mine = quad_corner(kp, c, ru, rv, lane & 3);
 #pragma unroll 1
   for (int tri = 0; tri < 2; ++tri) {
-    TriSetup t = tri == 0 ? tri_prepare(q[0], q[1], q[2], kp.Wm, kp.Hm) : tri_prepare(q[1], q[2], q[3], kp.Wm, kp.Hm);
-    if (!t.valid) continue;
-    const int wd = t.ni + 1, total = wd * (t.nj + 1);
-    const bool tieA = t.ties & 1u, tieB = t.ties & 2u, tieC = t.ties & 4u;
-    for (int item = lane; item < total; item += 32) {
-      const int dj = item / wd, di = item - dj * wd;
-      const long long wA = t.eA + (long long)di * t.sxA + (long long)dj * t.syA;
-      const long long wB = t.eB + (long long)di * t.sxB + (long long)dj * t.syB;
-      const long long wC = t.eC + (long long)di * t.sxC + (long long)dj * t.syC;
-      const bool in = (wA > 0 || (wA == 0 && tieA)) && (wB > 0 || (wB == 0 && tieB)) && (wC > 0 || (wC == 0 && tieC));
-      if (!in) continue;
-      float fB = (float)wB / t.farea, fC = (float)wC / t.farea;
-      float fA = (1.0f - fB) - fC;
-      float tx = (fA * t.txA + fB * t.txB) + fC * t.txC;
-      float ty = (fA * t.tyA + fB * t.tyB) + fC * t.tyC;
-      float z = (fA * t.zA + fB * t.zB) + fC * t.zC;
-      emit_fragment(tx, ty, z, (size_t)(t.j0 + dj) * kp.Wm + (size_t)(t.i0 + di), c.k, c.flags, rt);
-    }
+    const RVert A = shfl_corner(mine, tri), B = shfl_corner(mine, tri + 1), C = shfl_corner(mine, tri + 2);
+    __syncwarp();  // every lane is done with the previous set-up
+    if (lane == 0) tri_prepare(A, B, C, kp.Wm, kp.Hm, st);
+    __syncwarp();
+    raster_big_tri(kp, st, tri, c.k, c.flags, rt, lane);
   }
 }
 
@@ -312,11 +280,37 @@ struct QuadStore {
   int prefix[kRenderThreads + 1];  // exclusive prefix of the box pixel counts (0 for large / empty quads)
 };
 
-__device__ __forceinline__ void quad_store_tri(QuadStore& Q, int slot, int tri, const TriSmall& t) {
-  Q.e[tri][0][slot] = t.eA; Q.e[tri][1][slot] = t.eB; Q.e[tri][2][slot] = t.eC;
-  Q.sx[tri][0][slot] = t.sxA; Q.sx[tri][1][slot] = t.sxB; Q.sx[tri][2][slot] = t.sxC;
-  Q.sy[tri][0][slot] = t.syA; Q.sy[tri][1][slot] = t.syB; Q.sy[tri][2][slot] = t.syC;
-  Q.farea[tri][slot] = t.farea;
+__device__ __forceinline__ int edge32(int Px, int Py, int Qx, int Qy) {  // edge_fn(P, Q, X0, Y0), P and Q relative to (X0, Y0)
+  return (Qx - Px) * (0 - Py) - (Qy - Py) * (0 - Px);
+}
+__device__ __forceinline__ bool tie32(int Px, int Py, int Qx, int Qy) {
+  int dx = Qx - Px, dy = Qy - Py;
+  return dy > 0 || (dy == 0 && dx > 0);
+}
+// One triangle (corners A, B, C) of a small quad, everything relative to the quad's first pixel centre (X0, Y0): all
+// magnitudes stay below 2^14 + 2^10, so the int32 edge functions, their steps and the area equal the int64 ones of
+// tri_prepare() bit for bit. The set-up goes straight to slot `slot` of Q (so that only one triangle's is ever live);
+// returns the triangle's meta bits, ties (3) | swapped (1) | valid (1), and 0 for a degenerate triangle, which stores
+// nothing. Phase 2 takes the corner depths and texture coordinates from the swapped bit.
+__device__ __forceinline__ uint32_t tri_small_store(QuadStore& Q, int slot, int tri, int Ax, int Ay, int Bx, int By,
+                                                    int Cx, int Cy) {
+  int area = (Bx - Ax) * (Cy - Ay) - (By - Ay) * (Cx - Ax);
+  if (area == 0) return 0u;
+  uint32_t swapped = 0u;
+  if (area < 0) {  // same orientation fix as tri_prepare(): swap B and C
+    int ti = Bx; Bx = Cx; Cx = ti;
+    ti = By; By = Cy; Cy = ti;
+    area = -area;
+    swapped = 8u;
+  }
+  Q.farea[tri][slot] = (float)area;
+  Q.e[tri][0][slot] = edge32(Bx, By, Cx, Cy);
+  Q.e[tri][1][slot] = edge32(Cx, Cy, Ax, Ay);
+  Q.e[tri][2][slot] = edge32(Ax, Ay, Bx, By);
+  Q.sx[tri][0][slot] = -256 * (Cy - By); Q.sx[tri][1][slot] = -256 * (Ay - Cy); Q.sx[tri][2][slot] = -256 * (By - Ay);
+  Q.sy[tri][0][slot] = 256 * (Cx - Bx); Q.sy[tri][1][slot] = 256 * (Ax - Cx); Q.sy[tri][2][slot] = 256 * (Bx - Ax);
+  return (tie32(Bx, By, Cx, Cy) ? 1u : 0u) | (tie32(Cx, Cy, Ax, Ay) ? 2u : 0u) | (tie32(Ax, Ay, Bx, By) ? 4u : 0u) |
+         swapped | 16u;
 }
 
 // K6a, gen_indexmap.vert:62-81 for one visible surfel k whose centre projects to (x, y, z) under the data image's
@@ -360,7 +354,9 @@ __global__ void __launch_bounds__(kRenderThreads, kMinBlocks) k_render_scatter(K
   __shared__ int s_warp_cnt[kRenderThreads / 32];
   __shared__ int s_nbig;
   __shared__ uint16_t s_big[kRenderThreads];
-  __shared__ uint32_t s_fq[kRenderThreads / 32][kFragQueue];
+  // per warp: the fragment queue of the small quads, then the triangle set-up of its large quads (raster_big)
+  __shared__ __align__(8) uint32_t s_fq[kRenderThreads / 32][kFragQueue];
+  static_assert(sizeof(TriSetup) <= sizeof(s_fq[0]) && sizeof(s_fq[0]) % 8 == 0, "a warp's queue holds a TriSetup");
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   if (tid == 0) s_nbig = 0;
   const uint32_t k = blockIdx.x * blockDim.x + tid;
@@ -429,8 +425,11 @@ __global__ void __launch_bounds__(kRenderThreads, kMinBlocks) k_render_scatter(K
   if (tid < total) {
     c.px = c_f[0][tid]; c.py = c_f[1][tid]; c.pz = c_f[2][tid]; c.nx = c_f[3][tid];
     c.ny = c_f[4][tid]; c.nz = c_f[5][tid]; c.r = c_f[6][tid]; c.cx = c_f[7][tid];
+    V3 ru, rv;
+    quad_axes(c, ru, rv);
     RVert q[4];
-    quad_corners(kp, c, q);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) q[i] = quad_corner(kp, c, ru, rv, i);
     // pixel bounding box of the quad (union of the boxes of its two triangles), clamped to the image
     long long minX = min(min(q[0].X, q[1].X), min(q[2].X, q[3].X)), maxX = max(max(q[0].X, q[1].X), max(q[2].X, q[3].X));
     long long minY = min(min(q[0].Y, q[1].Y), min(q[2].Y, q[3].Y)), maxY = max(max(q[0].Y, q[1].Y), max(q[2].Y, q[3].Y));
@@ -450,12 +449,15 @@ __global__ void __launch_bounds__(kRenderThreads, kMinBlocks) k_render_scatter(K
         small = small && dx > -kSmallSpan && dx < kSmallSpan && dy > -kSmallSpan && dy < kSmallSpan;
       }
       if (small) {
-        const TriSmall t0 = tri_small(q[0], q[1], q[2], X0, Y0), t1 = tri_small(q[1], q[2], q[3], X0, Y0);
-        const uint32_t m0 = t0.valid ? (t0.ties | (t0.swapped ? 8u : 0u) | 16u) : 0u;
-        const uint32_t m1 = t1.valid ? (t1.ties | (t1.swapped ? 8u : 0u) | 16u) : 0u;
+        int rx[4], ry[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          rx[i] = (int)(q[i].X - X0);
+          ry[i] = (int)(q[i].Y - Y0);
+        }
+        const uint32_t m0 = tri_small_store(Q, tid, 0, rx[0], ry[0], rx[1], ry[1], rx[2], ry[2]);
+        const uint32_t m1 = tri_small_store(Q, tid, 1, rx[1], ry[1], rx[2], ry[2], rx[3], ry[3]);
         if (m0 | m1) {
-          if (t0.valid) quad_store_tri(Q, tid, 0, t0);
-          if (t1.valid) quad_store_tri(Q, tid, 1, t1);
           Q.z[0][tid] = q[0].z; Q.z[1][tid] = q[1].z; Q.z[2][tid] = q[2].z; Q.z[3][tid] = q[3].z;
           Q.box[tid] = (uint32_t)i0 | ((uint32_t)j0 << 16);
           Q.meta[tid] = (uint32_t)ni | ((uint32_t)nj << 8) | (m0 << 16) | (m1 << 21) | (c_flags[tid] << 26);
@@ -562,25 +564,25 @@ __global__ void __launch_bounds__(kRenderThreads, kMinBlocks) k_render_scatter(K
       __syncwarp();
       // phase 2
       for (int i0q = 0; i0q < qn; i0q += 32 * kFragBatch) {
-        uint32_t ent[kFragBatch];
+        // per fragment only the queue entry, the pixel and the fetched key stay live; the key image is chosen again from
+        // the surfel class when it is used. The pixel index fits 32 bits: Q.box holds i0 and j0 in 16 bits each, which
+        // already limits the model image to 65536 x 65536 pixels, so the index is at most 2^32 - 1.
+        uint32_t ent[kFragBatch], pixs[kFragBatch];
         unsigned long long cur[kFragBatch];
-        unsigned long long* img[kFragBatch];
-        size_t pixs[kFragBatch];
 #pragma unroll
         for (int b2 = 0; b2 < kFragBatch; ++b2) {
           const int i = i0q + 32 * b2 + lane;
           ent[b2] = i < qn ? fq[i] : 0xffffffffu;
           cur[b2] = 0ull;
-          img[b2] = nullptr;
-          pixs[b2] = 0;
+          pixs[b2] = 0u;
           if (ent[b2] != 0xffffffffu) {
             const int sl = (int)(ent[b2] & 255u);
             const uint32_t box = Q.box[sl];
-            pixs[b2] = (size_t)((int)(box >> 16) + (int)((ent[b2] >> 12) & 7u)) * kp.Wm + (size_t)((int)(box & 0xffffu) + (int)((ent[b2] >> 8) & 15u));
+            pixs[b2] = ((box >> 16) + ((ent[b2] >> 12) & 7u)) * (uint32_t)kp.Wm + ((box & 0xffffu) + ((ent[b2] >> 8) & 15u));
             const uint32_t cls = (Q.meta[sl] >> 26) & 3u;  // 1 old, 2 new, 3 both (an old surfel re-observed recently)
             if (plain && cls != 3u) {
-              img[b2] = (cls & 1u) ? rt.key_old : rt.key_new;
-              if (img[b2]) cur[b2] = img[b2][pixs[b2]];
+              const unsigned long long* img = (cls & 1u) ? rt.key_old : rt.key_new;
+              if (img) cur[b2] = img[pixs[b2]];
             }
           }
         }
@@ -598,19 +600,21 @@ __global__ void __launch_bounds__(kRenderThreads, kMinBlocks) k_render_scatter(K
           const float farea = Q.farea[tri][sl];
           const float fB = (float)wB / farea, fC = (float)wC / farea;
           const float fA = (1.0f - fB) - fC;
-          const float txA = (cA & 1) ? 1.0f : -1.0f, txB = (cB & 1) ? 1.0f : -1.0f, txC = (cC & 1) ? 1.0f : -1.0f;
-          const float tyA = (cA & 2) ? 1.0f : -1.0f, tyB = (cB & 2) ? 1.0f : -1.0f, tyC = (cC & 2) ? 1.0f : -1.0f;
+          const float txA = corner_tx(cA), txB = corner_tx(cB), txC = corner_tx(cC);
+          const float tyA = corner_ty(cA), tyB = corner_ty(cB), tyC = corner_ty(cC);
           const float tx = (fA * txA + fB * txB) + fC * txC;
           const float ty = (fA * tyA + fB * tyB) + fC * tyC;
           const float z = (fA * Q.z[cA][sl] + fB * Q.z[cB][sl]) + fC * Q.z[cC][sl];
-          if (plain && ((mt >> 26) & 3u) != 3u) {
-            if (!img[b2]) continue;
+          const uint32_t cls = (mt >> 26) & 3u;
+          if (plain && cls != 3u) {
+            unsigned long long* img = (cls & 1u) ? rt.key_old : rt.key_new;
+            if (!img) continue;
             if (tx * tx + ty * ty > 1.0f) continue;   // outside the disc (render_surfels.frag:22-28)
             if (!(z >= 0.0f && z <= 1.0f)) continue;  // near / far clip
             const unsigned long long d = (unsigned long long)depth24(z);
             if (d >= kDepthClear) continue;           // GL_LESS against the cleared depth
             const unsigned long long key = (d << 40) | Q.k[sl];
-            if (key < cur[b2]) atomicMin(img[b2] + pixs[b2], key);
+            if (key < cur[b2]) atomicMin(img + pixs[b2], key);
           } else {
             emit_fragment(tx, ty, z, pixs[b2], Q.k[sl], mt >> 26, rt);
           }
@@ -627,7 +631,7 @@ __global__ void __launch_bounds__(kRenderThreads, kMinBlocks) k_render_scatter(K
     cb.px = c_f[0][slot]; cb.py = c_f[1][slot]; cb.pz = c_f[2][slot]; cb.nx = c_f[3][slot];
     cb.ny = c_f[4][slot]; cb.nz = c_f[5][slot]; cb.r = c_f[6][slot]; cb.cx = c_f[7][slot];
     cb.k = Q.k[slot]; cb.flags = c_flags[slot];
-    raster_big(kp, cb, rt, lane);
+    raster_big(kp, cb, rt, lane, *reinterpret_cast<TriSetup*>(s_fq[warp]));
   }
 }
 
@@ -638,8 +642,8 @@ void launch_render_scatter(const Launch& L, const KParams& kp, SurfelPlanes s, c
   {
     ScopedKernel sk(L, K_RENDER_SCATTER);
     const unsigned grid = (n_upper + kRenderThreads - 1) / kRenderThreads;
-    // 4 resident blocks per SM (64 registers, 46.6 KB shared memory): the kernel is bound by instruction issue and
-    // dependent L2 round trips, so occupancy is held at the cost of some spills (microbench.py times the launch)
+    // 4 resident blocks per SM (64 registers, no local memory, 46.6 KB shared memory): the kernel is bound by
+    // instruction issue and dependent L2 round trips (renderbench.py times both instances)
     if (index)
       k_render_scatter<4, true><<<grid, kRenderThreads, 0, L.stream>>>(kp, s, n_dev, live, M, conf_thr, t_thr, emit_old,
                                                                        emit_new, lequal, t, *index);
