@@ -99,6 +99,7 @@ int sb_create(const sb_params* p, int device, sb_ctx** out);       /* SurfelMapp
 int sb_destroy(sb_ctx* ctx);
 int sb_reset(sb_ctx* ctx);                                         /* SurfelMapping::reset / SurfelMap::reset, SurfelMap.cpp:473 */
 int sb_set_params(sb_ctx* ctx, const sb_params* p);                /* SurfelMapping::setParameters, SurfelMapping.cpp:68 */
+int sb_get_params(const sb_ctx* ctx, sb_params* p);               /* the parameters in effect (e.g. after sb_state_load) */
 const char* sb_last_error(const sb_ctx* ctx);
 int sb_synchronize(sb_ctx* ctx);
 int sb_device_count(void);
@@ -227,6 +228,27 @@ int sb_slam_frame(sb_ctx* ctx, int which, sb_frame** out); /* getCurrentFrame / 
  * [12] surfels dropped because the HBM cache of extracted submap tiles (16 M surfels) was full -- the reference's
  * host-side submapCache_ is unbounded; sb_last_error carries the message */
 int sb_get_statistics(sb_ctx* ctx, double stats[16]);
+
+/* ---- checkpoint / resume (no counterpart in the reference: its Posegraph::save/load are empty stubs) --------------
+ * A checkpoint holds everything the next scan depends on: the live surfels in order, the used part of the HBM tile pool
+ * with its records and bookkeeping, both pose tables, the device pose block, the SLAM poses, statistics, the seven frames,
+ * the loop-closure state, the sb_params and the loop parameters. N scans, save, load into a fresh context, M scans give
+ * the bits of N + M scans without a break. Format (DESIGN.md section 9): little-endian header (magic, format version,
+ * SB_VERSION, sizeof(sb_surfel), pose capacity, image sizes, total size, sb_params, loop parameters), length-prefixed
+ * sections, a 64-bit digest of everything before it. save(load(save(x))) == save(x) byte for byte.
+ *  - sb_state_save does not change the context; sb_state_size is the exact size of a checkpoint taken now.
+ *  - sb_state_load restores into any context created with the same image sizes, applies the saved sb_params (validated as
+ *    sb_set_params does) and drops the render memo. A bad header, a size mismatch or a truncated buffer returns
+ *    SB_ERR_INVALID before anything changes; a digest mismatch returns SB_ERR_INVALID with the context reset (sb_reset).
+ *  - a save or a load that goes ahead drops the scans staged by sb_prefetch_scan (a checkpoint neither carries nor consumes
+ *    them); a call refused for its arguments, a too small buffer or a bad header leaves them staged; a load refused for
+ *    its digest has dropped them with the rest of the context's state.
+ *  - both return SB_ERR_STATE while a multi-GPU exchange is set up.
+ *  - a map with surfels removed in place is restored dense: only the physical slot ids that sb_map_update_debug reports
+ *    after the next sb_process_scan can differ. */
+int sb_state_size(sb_ctx* ctx, uint64_t* bytes);
+int sb_state_save(sb_ctx* ctx, void* dst, uint64_t cap, uint64_t* written);
+int sb_state_load(sb_ctx* ctx, const void* src, uint64_t n);
 
 /* ---- per-kernel device time (CUDA events on the context's stream around every launch; off by default) ------------ */
 int sb_profile_enable(sb_ctx* ctx, int on);

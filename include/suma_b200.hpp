@@ -14,7 +14,9 @@
 #ifndef SUMA_B200_HPP_
 #define SUMA_B200_HPP_
 
+#include <cstddef>
 #include <cstdint>
+#include <cstdio>
 #include <cstring>
 #include <map>
 #include <memory>
@@ -174,6 +176,8 @@ class Context {
     check(sb_set_params(ctx_, &p.raw()), ctx_, "setParameters");
     params_ = p;
   }
+  /** the parameters the library already holds (after sb_state_load) */
+  void adoptParameters(const ParameterList& p) { params_ = p; }
 
  private:
   ParameterList params_;
@@ -548,6 +552,46 @@ class SurfelMapping {
     return st;
   }
   const ContextPtr& context() const { return ctx_; }
+
+  /** Checkpoint of the whole mapping session (sb_state_save; no counterpart in the reference, whose
+   * Posegraph::save/load are empty stubs): loading it into a SurfelMapping of the same image size and continuing gives
+   * the bits of an uninterrupted run. */
+  std::vector<uint8_t> saveState() const {
+    uint64_t n = 0;
+    check(sb_state_size(ctx_->get(), &n), ctx_->get(), "SurfelMapping::saveState");
+    std::vector<uint8_t> blob(static_cast<size_t>(n));
+    check(sb_state_save(ctx_->get(), blob.data(), n, &n), ctx_->get(), "SurfelMapping::saveState");
+    blob.resize(static_cast<size_t>(n));
+    return blob;
+  }
+  /** Restores a saveState() checkpoint and the parameters it carries. The odometry list of this mirror
+   * (getOptimizedPoses) restarts at the load. */
+  void loadState(const std::vector<uint8_t>& blob) {
+    check(sb_state_load(ctx_->get(), blob.empty() ? nullptr : blob.data(), blob.size()), ctx_->get(),
+          "SurfelMapping::loadState");
+    sb_params p;
+    check(sb_get_params(ctx_->get(), &p), ctx_->get(), "SurfelMapping::loadState");
+    ctx_->adoptParameters(ParameterList(p));
+    trajectory_.clear();
+  }
+  /** file variants, in the spirit of the reference's storePoseGraph(filename) */
+  void saveState(const std::string& filename) const {
+    const std::vector<uint8_t> blob = saveState();
+    FILE* f = std::fopen(filename.c_str(), "wb");
+    if (!f) throw std::runtime_error("SurfelMapping::saveState: cannot open " + filename);
+    const bool ok = std::fwrite(blob.data(), 1, blob.size(), f) == blob.size();
+    if (std::fclose(f) != 0 || !ok) throw std::runtime_error("SurfelMapping::saveState: cannot write " + filename);
+  }
+  void loadState(const std::string& filename) {
+    FILE* f = std::fopen(filename.c_str(), "rb");
+    if (!f) throw std::runtime_error("SurfelMapping::loadState: cannot open " + filename);
+    std::vector<uint8_t> blob;
+    uint8_t buf[1 << 16];
+    size_t k;
+    while ((k = std::fread(buf, 1, sizeof(buf), f)) > 0) blob.insert(blob.end(), buf, buf + k);
+    std::fclose(f);
+    loadState(blob);
+  }
 
  private:
   Frame::Ptr slam_frame(int which) {

@@ -116,6 +116,7 @@ def lib(build_if_missing=True):
         "sb_default_params": [C.POINTER(Params)],
         "sb_create": [C.POINTER(Params), C.c_int, pv],
         "sb_destroy": [vp], "sb_reset": [vp], "sb_set_params": [vp, C.POINTER(Params)], "sb_synchronize": [vp],
+        "sb_get_params": [vp, C.POINTER(Params)],
         "sb_frame_create": [vp, C.c_int, C.c_int, pv], "sb_frame_destroy": [vp], "sb_frame_copy": [vp, vp],
         "sb_frame_download": [vp, C.c_int, vp], "sb_frame_upload": [vp, C.c_int, vp],
         "sb_frame_size": [vp, C.POINTER(C.c_int), C.POINTER(C.c_int)],
@@ -144,6 +145,8 @@ def lib(build_if_missing=True):
         "sb_comm_set_callback": [vp, vp, vp, C.c_int, C.c_int],
         "sb_profile_enable": [vp, C.c_int], "sb_profile_collect": [vp, pd, C.POINTER(C.c_uint64), C.c_int],
         "sb_profile_kernels": [],
+        "sb_state_size": [vp, C.POINTER(C.c_uint64)], "sb_state_save": [vp, vp, C.c_uint64, C.POINTER(C.c_uint64)],
+        "sb_state_load": [vp, vp, C.c_uint64],
     }
     for name, args in sig.items():
         fn = getattr(L, name)
@@ -162,7 +165,8 @@ def lib(build_if_missing=True):
 
 
 EXPORTED_SYMBOLS = [
-    "sb_default_params", "sb_create", "sb_destroy", "sb_reset", "sb_set_params", "sb_last_error", "sb_synchronize",
+    "sb_default_params", "sb_create", "sb_destroy", "sb_reset", "sb_set_params", "sb_get_params", "sb_last_error",
+    "sb_synchronize",
     "sb_device_count", "sb_stream", "sb_launch_count", "sb_frame_create", "sb_frame_destroy", "sb_frame_copy",
     "sb_frame_download", "sb_frame_upload", "sb_frame_size", "sb_preprocess", "sb_map_render", "sb_map_render_active",
     "sb_map_render_inactive", "sb_map_render_composed", "sb_map_frame", "sb_icp_jacobian", "sb_icp_unpack",
@@ -172,7 +176,7 @@ EXPORTED_SYMBOLS = [
     "sb_get_statistics", "sb_comm_export", "sb_comm_init", "sb_comm_shutdown", "sb_comm_set_callback",
     "sb_profile_enable", "sb_default_loop_params", "sb_set_loop_closure", "sb_get_loop_info", "sb_get_loop_edges",
     "sb_set_current_pose", "sb_integrate_loop_closures",
-    "sb_profile_kernels", "sb_profile_name", "sb_profile_collect",
+    "sb_profile_kernels", "sb_profile_name", "sb_profile_collect", "sb_state_size", "sb_state_save", "sb_state_load",
 ]
 
 
@@ -256,6 +260,12 @@ class Context:
         ms = np.zeros(n); cnt = np.zeros(n, np.uint64)
         self.check(lib().sb_profile_collect(self.h, _dp(ms), cnt.ctypes.data_as(C.POINTER(C.c_uint64)), n), "profile")
         return {lib().sb_profile_name(i).decode(): (float(ms[i]), int(cnt[i])) for i in range(n) if cnt[i]}
+
+    def get_params(self):
+        """the parameters in effect (sb_get_params)"""
+        p = Params()
+        self.check(lib().sb_get_params(self.h, C.byref(p)), "get_params")
+        return p
 
     def set_params(self, params):
         self.check(lib().sb_set_params(self.h, C.byref(params)), "set_params")
@@ -650,3 +660,30 @@ class SurfelMapping:
 
     def reset(self):
         self.ctx.check(lib().sb_reset(self.ctx.h), "reset")
+
+    def save_state(self):
+        """The whole state of the mapping session as bytes (sb_state_save): loading it into a context of the same image
+        size and continuing gives the bits of an uninterrupted run. Scans staged by prefetch_scan_raw are dropped."""
+        n = C.c_uint64(0)
+        self.ctx.check(lib().sb_state_size(self.ctx.h, C.byref(n)), "state_size")
+        buf = np.empty(n.value, np.uint8)
+        w = C.c_uint64(0)
+        self.ctx.check(lib().sb_state_save(self.ctx.h, _vp(buf), n.value, C.byref(w)), "state_save")
+        return buf[:w.value].tobytes()
+
+    def load_state(self, blob):
+        """Restores a save_state() checkpoint, its parameters included (sb_state_load). Raises SumaError on a blob of
+        another format, image size or a corrupted one (after which the context is reset)."""
+        a = np.frombuffer(blob, np.uint8)
+        self.ctx.check(lib().sb_state_load(self.ctx.h, _vp(a) if a.size else None, a.size), "state_load")
+        self.ctx.params = self.ctx.get_params()
+
+    def save_state_file(self, path):
+        data = self.save_state()
+        with open(path, "wb") as f:
+            f.write(data)
+        return len(data)
+
+    def load_state_file(self, path):
+        with open(path, "rb") as f:
+            self.load_state(f.read())

@@ -178,6 +178,12 @@ struct sb_ctx {
   void* comm_cb_user = nullptr;
   int row_begin = 0, row_end = 0;
   std::vector<void*> peer_ptrs;
+
+  // ---- checkpoints (sb_state_save / sb_state_load): a pinned double buffer for the chunked copies, its two events and the
+  // device digest accumulator; created on first use, so contexts that never checkpoint pay nothing
+  PinnedPtr<uint8_t> state_stage;
+  cudaEvent_t state_ev[2] = {nullptr, nullptr};
+  DevPtr<unsigned long long> state_acc;
 };
 
 namespace {
@@ -1288,6 +1294,8 @@ int sb_destroy(sb_ctx* c) {
     if (sl.released) cudaEventDestroy(sl.released);
   }
   if (c->copy_stream) cudaStreamDestroy(c->copy_stream);
+  for (cudaEvent_t e : c->state_ev)
+    if (e) cudaEventDestroy(e);
   for (auto& r : c->prof.recs) {  // events of the per-kernel profiler (sb_profile_*)
     cudaEventDestroy(r.e0);
     cudaEventDestroy(r.e1);
@@ -1313,6 +1321,12 @@ int sb_set_params(sb_ctx* c, const sb_params* p) {
   c->p = *p;
   derive(c);
   c->memo.clear();
+  return SB_OK;
+}
+
+int sb_get_params(const sb_ctx* c, sb_params* p) {
+  if (!c || !p) return SB_ERR_INVALID;
+  *p = c->p;
   return SB_OK;
 }
 
@@ -1967,6 +1981,694 @@ int sb_comm_shutdown(sb_ctx* c) {
   c->peer_ptrs.clear();
   c->comm_on = false;
   return SB_OK;
+}
+
+}  // extern "C"
+
+// =========================================================================================================
+// Checkpoints: sb_state_size / sb_state_save / sb_state_load (no counterpart in the reference, whose Posegraph::save/load
+// are empty stubs). DESIGN.md section 9 lists which member of sb_ctx is saved, derived or context-local, and the format.
+// =========================================================================================================
+namespace {
+
+static_assert(__BYTE_ORDER__ == __ORDER_LITTLE_ENDIAN__, "checkpoints are written little-endian");
+const char kStateMagic[8] = {'S', 'B', 'S', 'T', 'A', 'T', 'E', '\0'};
+constexpr uint32_t kStateFormat = 1;
+constexpr size_t kStageBytes = 16u << 20;  // one half of the pinned double buffer
+enum StateSection : uint32_t { S_HOST = 1, S_LOOP, S_POSES, S_RESULT, S_TILES, S_SURFELS, S_POOL, S_FRAMES };
+
+#define SB_PARAM_FIELDS(X)                                                                                              \
+  X(data_width) X(data_height) X(data_fov_up) X(data_fov_down) X(min_depth) X(max_depth) X(model_width)                 \
+  X(model_height) X(model_fov_up) X(model_fov_down) X(model_min_depth) X(model_max_depth) X(max_iterations)            \
+  X(stopping_threshold) X(delta) X(icp_max_distance) X(icp_max_angle) X(weighting) X(factor) X(initialize_identity)     \
+  X(bilinear_sampling) X(fallback_mode) X(fallback_max_distance) X(fallback_max_angle) X(compose_rendering)             \
+  X(max_loop_closure_distance) X(min_radius) X(max_radius) X(max_angle) X(map_max_distance) X(map_max_angle)            \
+  X(unstable_age) X(confidence_mode) X(confidence_threshold) X(p_stable) X(p_prior) X(sigma_angle) X(sigma_distance)    \
+  X(use_stability) X(active_timestamps) X(max_weight) X(weighting_scheme) X(averaging_scheme) X(update_always)          \
+  X(submap_dimension) X(submap_extent) X(partial_extraction) X(label_offset_quirk) X(render_after_update)
+#define SB_LOOP_PARAM_FIELDS(X)                                                                                         \
+  X(search_distance) X(min_trajectory_distance) X(min_verifications) X(residual_threshold) X(outlier_threshold)         \
+  X(valid_threshold) X(delta_timestamp)
+
+// Field-by-field little-endian writer / reader: no padding byte of a C++ struct ever reaches a checkpoint, so that
+// saving a loaded checkpoint reproduces it byte for byte.
+struct Writer {
+  std::vector<uint8_t> b;
+  template <class T>
+  void put(const T& v) {
+    const uint8_t* p = reinterpret_cast<const uint8_t*>(&v);
+    b.insert(b.end(), p, p + sizeof(T));
+  }
+  void bytes(const void* p, size_t n) {
+    const uint8_t* q = static_cast<const uint8_t*>(p);
+    b.insert(b.end(), q, q + n);
+  }
+  void align8() { b.resize((b.size() + 7) & ~size_t(7), 0); }
+  size_t open(uint32_t id) {  // section header: id, 0, payload length (patched by close)
+    put(id); put(uint32_t(0)); put(uint64_t(0));
+    return b.size();
+  }
+  void close(size_t start) {
+    align8();
+    const uint64_t len = b.size() - start;
+    memcpy(&b[start - 8], &len, 8);
+  }
+};
+struct Reader {
+  const uint8_t* p;
+  size_t n, off = 0;
+  bool ok = true;
+  template <class T>
+  T get() {
+    T v{};
+    if (!ok || n - off < sizeof(T)) { ok = false; return v; }
+    memcpy(&v, p + off, sizeof(T));
+    off += sizeof(T);
+    return v;
+  }
+  void bytes(void* dst, size_t k) {
+    if (!ok || n - off < k) { ok = false; return; }
+    memcpy(dst, p + off, k);
+    off += k;
+  }
+  uint32_t count(size_t elem) {  // a length prefix that cannot claim more elements than bytes remain
+    uint32_t k = get<uint32_t>();
+    if (ok && (uint64_t)k * elem > n - off) ok = false;
+    return ok ? k : 0;
+  }
+  void align8() {
+    size_t a = (off + 7) & ~size_t(7);
+    if (a > n) ok = false; else off = a;
+  }
+};
+
+namespace lp = suma_b200::loop;
+
+// Everything a checkpoint holds except the three device-resident bulk sections (surfels, tile pool, frames).
+struct StateImage {
+  sb_params p;
+  uint32_t timestamp = 0, trackLoss = 0;
+  double currentPose[16], lastPose[16], currentPose_old[16], currentPose_new[16], lastIncrement[16], lastPose_old[16];
+  float confidence_threshold = 0.f, log_unstable_slam = 0.f;
+  double stats[16];
+  uint32_t cur_has_semantics = 0, last_has_semantics = 0, close_loops = 0;
+  uint32_t n_live = 0, map_timestamp = 0, pose_ref_end = 0, n_updated = 0, n_new = 0;
+  int32_t origin_i = 0, origin_j = 0;
+  std::vector<std::pair<int32_t, int32_t>> extraction;
+  std::vector<std::pair<std::pair<int32_t, int32_t>, DevTile>> tiles;
+  uint32_t n_slots = 0, tiles_pending = 0, pool_end = 0;
+  std::vector<float> poses, poses_inv;  // the used entries of the device pose tables
+  ResultBlock result;
+  std::vector<uint2> tile_rec;
+  lp::State loop;
+};
+
+void put_m4(Writer& w, const lp::M4& m) { w.bytes(m.m, sizeof(m.m)); }
+lp::M4 get_m4(Reader& r) {
+  lp::M4 m;
+  r.bytes(m.m, sizeof(m.m));
+  return m;
+}
+void put_edges(Writer& w, const std::vector<lp::Edge>& E) {
+  w.put((uint32_t)E.size());
+  for (const lp::Edge& e : E) { w.put(e.from); w.put(e.to); put_m4(w, e.rel); }
+}
+std::vector<lp::Edge> get_edges(Reader& r) {
+  std::vector<lp::Edge> E(r.count(136));
+  for (lp::Edge& e : E) { e.from = r.get<int32_t>(); e.to = r.get<int32_t>(); e.rel = get_m4(r); }
+  return E;
+}
+void put_result(Writer& w, const lp::OptResult& o) {
+  w.put(o.error); w.put(o.residual); w.put(o.inlier_residual);
+  w.put(o.inlier); w.put(o.outlier); w.put(o.valid); w.put(o.invalid); w.put(o.outlier_ratio);
+  put_m4(w, o.pose);
+}
+lp::OptResult get_result(Reader& r) {
+  lp::OptResult o;
+  o.error = r.get<double>(); o.residual = r.get<double>(); o.inlier_residual = r.get<double>();
+  o.inlier = r.get<uint32_t>(); o.outlier = r.get<uint32_t>(); o.valid = r.get<uint32_t>(); o.invalid = r.get<uint32_t>();
+  o.outlier_ratio = r.get<float>();
+  o.pose = get_m4(r);
+  return o;
+}
+
+void write_header(Writer& w, const StateImage& s, uint64_t total) {
+  w.bytes(kStateMagic, 8);
+  w.put(kStateFormat); w.put((uint32_t)SB_VERSION); w.put((uint32_t)sizeof(sb_surfel)); w.put(kMaxPoses);
+  w.put(s.p.data_width); w.put(s.p.data_height); w.put(s.p.model_width); w.put(s.p.model_height);
+  w.put(total);
+#define X(f) w.put(s.p.f);
+  SB_PARAM_FIELDS(X)
+#undef X
+#define X(f) w.put(s.loop.p.f);
+  SB_LOOP_PARAM_FIELDS(X)
+#undef X
+  w.align8();
+}
+
+void write_host_sections(Writer& w, const StateImage& s) {
+  size_t o = w.open(S_HOST);
+  w.put(s.timestamp);
+  for (const double* m : {s.currentPose, s.lastPose, s.currentPose_old, s.currentPose_new, s.lastIncrement, s.lastPose_old})
+    w.bytes(m, 128);
+  w.put(s.confidence_threshold); w.put(s.log_unstable_slam);
+  w.bytes(s.stats, sizeof(s.stats));
+  w.put(s.trackLoss); w.put(s.cur_has_semantics); w.put(s.last_has_semantics); w.put(s.close_loops);
+  w.put(s.n_live); w.put(s.map_timestamp); w.put(s.pose_ref_end); w.put(s.n_updated); w.put(s.n_new);
+  w.put(s.origin_i); w.put(s.origin_j);
+  w.put((uint32_t)s.extraction.size());
+  for (const auto& e : s.extraction) { w.put(e.first); w.put(e.second); }
+  w.put((uint32_t)s.tiles.size());
+  for (const auto& t : s.tiles) {
+    w.put(t.first.first); w.put(t.first.second);
+    w.put(t.second.slot); w.put((uint32_t)t.second.known); w.put(t.second.base); w.put(t.second.count);
+  }
+  w.put(s.n_slots); w.put(s.tiles_pending); w.put(s.pool_end);
+  w.close(o);
+
+  o = w.open(S_LOOP);
+  const lp::State& L = s.loop;
+  w.put((uint32_t)L.graph.poses.size());
+  for (const lp::M4& m : L.graph.poses) put_m4(w, m);
+  put_edges(w, L.graph.edges);
+  w.put((uint32_t)L.trajectory_distances.size());
+  w.bytes(L.trajectory_distances.data(), L.trajectory_distances.size() * sizeof(float));
+  put_result(w, L.result_new);
+  put_result(w, L.result_old);
+  put_edges(w, L.unverified);
+  put_edges(w, L.verified);
+  w.put((uint32_t)L.already_verified); w.put(L.time_without_loop_closure); w.put(L.loop_count);
+  w.put((uint32_t)L.found_candidate); w.put((uint32_t)L.use_candidate); w.put((uint32_t)L.optimisation_requested);
+  w.put(L.last_added_candidate); w.put(L.candidates_tested); w.put(L.loop_edges_added);
+  w.put(L.stat_valid_ratio); w.put(L.stat_outlier_ratio); w.put(L.stat_rel_error);
+  w.put(L.before_id); w.put(L.before_loop_count); put_m4(w, L.before_pose); w.put((uint64_t)L.requested_size);
+  w.close(o);
+
+  o = w.open(S_POSES);
+  w.put((uint32_t)(s.poses.size() / 16));
+  w.bytes(s.poses.data(), s.poses.size() * 4);
+  w.bytes(s.poses_inv.data(), s.poses_inv.size() * 4);
+  w.close(o);
+
+  o = w.open(S_RESULT);
+  w.bytes(&s.result, sizeof(ResultBlock));
+  w.close(o);
+
+  o = w.open(S_TILES);
+  w.put((uint32_t)s.tile_rec.size());
+  for (const uint2& r : s.tile_rec) { w.put(r.x); w.put(r.y); }
+  w.close(o);
+}
+
+// Opens section `id` and returns its payload length (0 and r.ok = false when the next section is another one).
+uint64_t read_open(Reader& r, uint32_t id) {
+  const uint32_t got = r.get<uint32_t>();
+  r.get<uint32_t>();
+  const uint64_t len = r.get<uint64_t>();
+  if (!r.ok || got != id || len > r.n - r.off || (len & 7)) r.ok = false;
+  return r.ok ? len : 0;
+}
+bool read_close(Reader& r, size_t start, uint64_t len) {
+  r.align8();
+  return r.ok && r.off - start == len;
+}
+
+// Parses the header and the host sections; nullptr when they are well formed, otherwise the reason.
+const char* read_host(Reader& r, const sb_ctx* c, StateImage& s) {
+  char magic[8];
+  r.bytes(magic, 8);
+  if (!r.ok || memcmp(magic, kStateMagic, 8) != 0) return "not a checkpoint (bad magic)";
+  const uint32_t fmt = r.get<uint32_t>(), ver = r.get<uint32_t>(), ssz = r.get<uint32_t>(), mp = r.get<uint32_t>();
+  if (!r.ok) return "truncated header";
+  if (fmt != kStateFormat) return "unsupported checkpoint format version";
+  if (ver != SB_VERSION) return "checkpoint written by another library version (SB_VERSION)";
+  if (ssz != sizeof(sb_surfel) || mp != kMaxPoses) return "checkpoint written with another surfel size / pose capacity";
+  int32_t dims[4];
+  for (int32_t& d : dims) d = r.get<int32_t>();
+  const uint64_t total = r.get<uint64_t>();
+  if (!r.ok) return "truncated header";
+  if (dims[0] != c->p.data_width || dims[1] != c->p.data_height || dims[2] != c->p.model_width ||
+      dims[3] != c->p.model_height)
+    return "checkpoint image geometry differs from the context's";
+  if (total != r.n) return total > r.n ? "truncated checkpoint" : "checkpoint size does not match its header";
+  memset(&s.p, 0, sizeof(s.p));
+#define X(f) s.p.f = r.get<decltype(s.p.f)>();
+  SB_PARAM_FIELDS(X)
+#undef X
+#define X(f) s.loop.p.f = r.get<decltype(s.loop.p.f)>();
+  SB_LOOP_PARAM_FIELDS(X)
+#undef X
+  r.align8();
+  if (!r.ok) return "truncated header";
+  if (check_params(&s.p)) return "checkpoint parameters are not valid";
+  if (s.p.data_width != dims[0] || s.p.data_height != dims[1] || s.p.model_width != dims[2] || s.p.model_height != dims[3])
+    return "checkpoint parameters disagree with its image geometry";
+
+  uint64_t len = read_open(r, S_HOST);
+  size_t start = r.off;
+  s.timestamp = r.get<uint32_t>();
+  for (double* m : {s.currentPose, s.lastPose, s.currentPose_old, s.currentPose_new, s.lastIncrement, s.lastPose_old})
+    r.bytes(m, 128);
+  s.confidence_threshold = r.get<float>(); s.log_unstable_slam = r.get<float>();
+  r.bytes(s.stats, sizeof(s.stats));
+  s.trackLoss = r.get<uint32_t>(); s.cur_has_semantics = r.get<uint32_t>(); s.last_has_semantics = r.get<uint32_t>();
+  s.close_loops = r.get<uint32_t>();
+  s.n_live = r.get<uint32_t>(); s.map_timestamp = r.get<uint32_t>(); s.pose_ref_end = r.get<uint32_t>();
+  s.n_updated = r.get<uint32_t>(); s.n_new = r.get<uint32_t>();
+  s.origin_i = r.get<int32_t>(); s.origin_j = r.get<int32_t>();
+  s.extraction.resize(r.count(8));
+  for (auto& e : s.extraction) { e.first = r.get<int32_t>(); e.second = r.get<int32_t>(); }
+  s.tiles.resize(r.count(24));
+  for (auto& t : s.tiles) {
+    t.first.first = r.get<int32_t>(); t.first.second = r.get<int32_t>();
+    t.second.slot = r.get<uint32_t>(); t.second.known = r.get<uint32_t>() != 0;
+    t.second.base = r.get<uint32_t>(); t.second.count = r.get<uint32_t>();
+  }
+  s.n_slots = r.get<uint32_t>(); s.tiles_pending = r.get<uint32_t>(); s.pool_end = r.get<uint32_t>();
+  if (!read_close(r, start, len)) return "malformed state section";
+  // A digest is no signature: every field that later sizes a copy or indexes device memory is range-checked here.
+  if (s.n_live > kMaxSurfels || s.n_slots > kMaxTileSlots || s.pool_end > kTilePoolCap ||
+      s.extraction.size() > kMaxTileSlots || s.tiles.size() > kMaxTileSlots)
+    return "checkpoint exceeds the map / tile-pool capacity";
+  if (s.pose_ref_end > kMaxPoses) return "malformed map state (pose-table reference beyond the table)";
+  for (const auto& t : s.tiles)
+    if (t.second.slot >= s.n_slots) return "malformed tile table";
+
+  len = read_open(r, S_LOOP);
+  start = r.off;
+  lp::State& L = s.loop;
+  L.graph.poses.resize(r.count(128));
+  for (lp::M4& m : L.graph.poses) m = get_m4(r);
+  L.graph.edges = get_edges(r);
+  L.trajectory_distances.resize(r.count(4));
+  r.bytes(L.trajectory_distances.data(), L.trajectory_distances.size() * 4);
+  L.result_new = get_result(r);
+  L.result_old = get_result(r);
+  L.unverified = get_edges(r);
+  L.verified = get_edges(r);
+  L.already_verified = r.get<uint32_t>() != 0;
+  L.time_without_loop_closure = r.get<uint32_t>(); L.loop_count = r.get<uint32_t>();
+  L.found_candidate = r.get<uint32_t>() != 0; L.use_candidate = r.get<uint32_t>() != 0;
+  L.optimisation_requested = r.get<uint32_t>() != 0;
+  L.last_added_candidate = r.get<int32_t>(); L.candidates_tested = r.get<uint32_t>(); L.loop_edges_added = r.get<uint32_t>();
+  L.stat_valid_ratio = r.get<float>(); L.stat_outlier_ratio = r.get<float>(); L.stat_rel_error = r.get<float>();
+  L.before_id = r.get<int32_t>(); L.before_loop_count = r.get<uint32_t>(); L.before_pose = get_m4(r);
+  L.requested_size = (size_t)r.get<uint64_t>();
+  if (!read_close(r, start, len)) return "malformed loop-closure section";
+  if (L.graph.poses.empty() || L.trajectory_distances.empty() || L.requested_size > L.graph.poses.size() ||
+      (L.optimisation_requested && (L.before_id < 0 || (size_t)L.before_id >= L.graph.poses.size())))
+    return "malformed loop-closure section";
+  // the next scan's check reads graph pose and travelled distance timestamp - 1 (SurfelMapping.cpp:460-469)
+  if (s.close_loops && s.timestamp > 0 &&
+      (L.graph.poses.size() < s.timestamp || L.trajectory_distances.size() < s.timestamp))
+    return "malformed loop-closure section (graph shorter than the sequence)";
+  for (const std::vector<lp::Edge>* E : {&L.graph.edges, &L.unverified, &L.verified})
+    for (const lp::Edge& e : *E)
+      if (e.from < 0 || e.to < 0 || (size_t)e.from >= L.graph.poses.size() || (size_t)e.to >= L.graph.poses.size())
+        return "malformed loop-closure section (edge outside the graph)";
+
+  len = read_open(r, S_POSES);
+  start = r.off;
+  const uint32_t np = r.count(128);
+  if (np > kMaxPoses) return "malformed pose tables";
+  s.poses.resize((size_t)np * 16);
+  s.poses_inv.resize((size_t)np * 16);
+  r.bytes(s.poses.data(), s.poses.size() * 4);
+  r.bytes(s.poses_inv.data(), s.poses_inv.size() * 4);
+  if (!read_close(r, start, len)) return "malformed pose tables";
+
+  len = read_open(r, S_RESULT);
+  start = r.off;
+  r.bytes(&s.result, sizeof(ResultBlock));
+  if (!read_close(r, start, len)) return "malformed result block";
+  if (s.result.counts[0] != s.n_live || s.result.counts[5] != 0) return "malformed result block (surfel counts)";
+
+  len = read_open(r, S_TILES);
+  start = r.off;
+  s.tile_rec.resize(r.count(8));
+  for (uint2& t : s.tile_rec) { t.x = r.get<uint32_t>(); t.y = r.get<uint32_t>(); }
+  if (!read_close(r, start, len) || s.tile_rec.size() != s.n_slots) return "malformed tile records";
+  if ((s.n_slots ? s.tile_rec[s.n_slots - 1].x : 0u) != s.pool_end) return "malformed tile records";
+  // slot k holds [end of slot k - 1, rec[k].x), no more than the tile had surfels (or the extract cap allows)
+  for (uint32_t k = 0; k < s.n_slots; ++k) {
+    const uint32_t base = k ? s.tile_rec[k - 1].x : 0u;
+    if (s.tile_rec[k].x < base || s.tile_rec[k].x - base > std::min(s.tile_rec[k].y, kExtractCap))
+      return "malformed tile records";
+  }
+  for (const auto& t : s.tiles) {  // a tile already read back names exactly its slot's range
+    const uint32_t base = t.second.slot ? s.tile_rec[t.second.slot - 1].x : 0u;
+    if (t.second.known && (t.second.base != base || t.second.count != s.tile_rec[t.second.slot].x - base))
+      return "malformed tile table";
+  }
+  return nullptr;
+}
+
+// The device-resident bulk of a checkpoint: (section id, device ranges in blob order)
+struct DevRange {
+  void* p;
+  uint64_t bytes;
+};
+struct DevSection {
+  uint32_t id;
+  std::vector<DevRange> ranges;
+  uint64_t bytes() const {
+    uint64_t n = 0;
+    for (const DevRange& r : ranges) n += r.bytes;
+    return n;
+  }
+};
+const sb_frame* const* frame_roles(const sb_ctx* c, const sb_frame* out[7]) {
+  const sb_frame* f[7] = {c->cur, c->last, c->cur_model, c->last_model, c->f_old, c->f_new, c->f_comp};
+  for (int i = 0; i < 7; ++i) out[i] = f[i];
+  return out;
+}
+// surfels go through the (idle) scratch lanes T as one flat block; pool lanes and frames are copied where they are
+std::vector<DevSection> dev_sections(sb_ctx* c, uint32_t n_live, uint32_t pool_end) {
+  std::vector<DevSection> d(3);
+  d[0].id = S_SURFELS;
+  d[0].ranges.push_back(DevRange{c->T.p0, (uint64_t)n_live * 64});
+  d[1].id = S_POOL;
+  for (float4* lane : {c->pool.p0, c->pool.p1, c->pool.p2, c->pool.p3})
+    d[1].ranges.push_back(DevRange{lane, (uint64_t)pool_end * 16});
+  d[2].id = S_FRAMES;
+  const sb_frame* f[7];
+  frame_roles(c, f);
+  for (const sb_frame* fr : f) d[2].ranges.push_back(DevRange{fr->base.get(), (uint64_t)fr->d.W * fr->d.H * 48});
+  return d;
+}
+
+uint64_t host_digest(const uint8_t* b, uint64_t off, uint64_t len) {  // off, len: multiples of 8
+  uint64_t h = 0;
+  for (uint64_t i = 0; i < len; i += 8) {
+    uint64_t w;
+    memcpy(&w, b + off + i, 8);
+    h += state_word_hash((off + i) / 8, w);
+  }
+  return h;
+}
+
+int state_staging(sb_ctx* c) {
+  if (c->state_stage) return SB_OK;
+  void* h = nullptr;
+  SB_CUDA(c, cudaMallocHost(&h, 2 * kStageBytes));
+  c->state_stage.reset(static_cast<uint8_t*>(h));
+  for (cudaEvent_t& e : c->state_ev) SB_CUDA(c, cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+  SB_CUDA(c, dev_alloc(c->state_acc, sizeof(unsigned long long)));
+  return SB_OK;
+}
+
+// Device ranges -> host bytes, in chunks through the pinned double buffer: the copy of chunk i from the pinned buffer
+// to `dst` runs while chunk i + 1 crosses the bus.
+int copy_out(sb_ctx* c, const std::vector<DevRange>& ranges, uint8_t* dst) {
+  uint8_t* stage[2] = {c->state_stage.get(), c->state_stage.get() + kStageBytes};
+  uint8_t* prev_dst = nullptr;
+  size_t prev_n = 0;
+  int buf = 0;
+  for (const DevRange& r : ranges)
+    for (uint64_t o = 0; o < r.bytes; o += kStageBytes) {
+      const size_t n = (size_t)std::min<uint64_t>(kStageBytes, r.bytes - o);
+      SB_CUDA(c, cudaMemcpyAsync(stage[buf], static_cast<uint8_t*>(r.p) + o, n, cudaMemcpyDeviceToHost, c->stream));
+      SB_CUDA(c, cudaEventRecord(c->state_ev[buf], c->stream));
+      if (prev_dst) {
+        SB_CUDA(c, cudaEventSynchronize(c->state_ev[buf ^ 1]));
+        memcpy(prev_dst, stage[buf ^ 1], prev_n);
+      }
+      prev_dst = dst;
+      prev_n = n;
+      dst += n;
+      buf ^= 1;
+    }
+  if (prev_dst) {
+    SB_CUDA(c, cudaEventSynchronize(c->state_ev[buf ^ 1]));
+    memcpy(prev_dst, stage[buf ^ 1], prev_n);
+  }
+  return SB_OK;
+}
+
+// host bytes -> device ranges: the host fills one half while the other half crosses the bus
+int copy_in(sb_ctx* c, const std::vector<DevRange>& ranges, const uint8_t* src) {
+  uint8_t* stage[2] = {c->state_stage.get(), c->state_stage.get() + kStageBytes};
+  bool used[2] = {false, false};
+  int buf = 0;
+  for (const DevRange& r : ranges)
+    for (uint64_t o = 0; o < r.bytes; o += kStageBytes) {
+      const size_t n = (size_t)std::min<uint64_t>(kStageBytes, r.bytes - o);
+      if (used[buf]) SB_CUDA(c, cudaEventSynchronize(c->state_ev[buf]));
+      memcpy(stage[buf], src, n);
+      SB_CUDA(c, cudaMemcpyAsync(static_cast<uint8_t*>(r.p) + o, stage[buf], n, cudaMemcpyHostToDevice, c->stream));
+      SB_CUDA(c, cudaEventRecord(c->state_ev[buf], c->stream));
+      used[buf] = true;
+      src += n;
+      buf ^= 1;
+    }
+  // the next call starts filling the pinned halves again: both must have crossed the bus
+  for (int b = 0; b < 2; ++b)
+    if (used[b]) SB_CUDA(c, cudaEventSynchronize(c->state_ev[b]));
+  return SB_OK;
+}
+
+// digest of the pool lanes and the frames (the surfels' is computed by the pack / unpack kernel), at their blob offsets
+void digest_ranges(sb_ctx* c, const DevSection& s, uint64_t data_off) {
+  for (const DevRange& r : s.ranges) {
+    launch_state_digest(L_(c), r.p, r.bytes / 8, data_off / 8, c->state_acc);
+    data_off += r.bytes;
+  }
+}
+
+// Scans staged by sb_prefetch_scan are dropped: a checkpoint neither carries nor consumes them.
+int discard_prefetch(sb_ctx* c) {
+  if (!c->copy_stream) return SB_OK;
+  SB_CUDA(c, cudaStreamSynchronize(c->copy_stream));
+  SB_CUDA(c, cudaStreamSynchronize(c->stream));
+  for (auto& sl : c->prefetch) sl.valid = sl.in_use = sl.has_released = false;
+  return SB_OK;
+}
+
+// The state of a context between calls, as a checkpoint holds it (reads the small device blocks back).
+int capture(sb_ctx* c, StateImage& s) {
+  SB_CUDA(c, cudaStreamSynchronize(c->stream));
+  s.p = c->p;
+  s.timestamp = c->timestamp;
+  s.trackLoss = c->trackLoss;
+  memcpy(s.currentPose, c->currentPose, 128); memcpy(s.lastPose, c->lastPose, 128);
+  memcpy(s.currentPose_old, c->currentPose_old, 128); memcpy(s.currentPose_new, c->currentPose_new, 128);
+  memcpy(s.lastIncrement, c->lastIncrement, 128); memcpy(s.lastPose_old, c->lastPose_old, 128);
+  s.confidence_threshold = c->confidence_threshold;
+  s.log_unstable_slam = c->log_unstable_slam;
+  memcpy(s.stats, c->stats, sizeof(s.stats));
+  s.cur_has_semantics = c->cur_has_semantics; s.last_has_semantics = c->last_has_semantics;
+  s.close_loops = c->close_loops;
+  s.n_live = n_live(c);
+  s.map_timestamp = c->map_timestamp; s.pose_ref_end = c->pose_ref_end;
+  s.n_updated = c->n_updated; s.n_new = c->n_new;
+  s.origin_i = c->origin_i; s.origin_j = c->origin_j;
+  s.extraction = c->extraction;
+  s.tiles.assign(c->tiles.begin(), c->tiles.end());
+  s.n_slots = c->n_slots;
+  s.tiles_pending = c->tiles_pending;
+  s.tile_rec.resize(c->n_slots);
+  if (c->n_slots)
+    SB_CUDA(c, cudaMemcpy(s.tile_rec.data(), c->d_tile_rec, (size_t)c->n_slots * sizeof(uint2), cudaMemcpyDeviceToHost));
+  s.pool_end = c->n_slots ? s.tile_rec[c->n_slots - 1].x : 0u;
+  // the used entries of the pose tables: those the map can refer to, and any set beyond them through sb_map_set_pose
+  uint32_t np = pose_table_count(c);
+  for (uint32_t t = kMaxPoses; t > np; --t) {
+    const float* e = &c->h_poses[16 * (size_t)(t - 1)];
+    bool ident = true;
+    for (int i = 0; i < 16; ++i) ident = ident && e[i] == ((i % 5 == 0) ? 1.0f : 0.0f);
+    if (!ident) { np = t; break; }
+  }
+  s.poses.resize((size_t)np * 16);
+  s.poses_inv.resize((size_t)np * 16);
+  SB_CUDA(c, cudaMemcpy(s.poses.data(), c->poses, (size_t)np * 64, cudaMemcpyDeviceToHost));
+  SB_CUDA(c, cudaMemcpy(s.poses_inv.data(), c->poses_inv, (size_t)np * 64, cudaMemcpyDeviceToHost));
+  SB_CUDA(c, cudaMemcpy(&s.result, c->res, sizeof(ResultBlock), cudaMemcpyDeviceToHost));
+  s.result.counts[0] = s.n_live;  // the map is restored dense: its physical end is the live count, no dead slots
+  s.result.counts[5] = 0;
+  s.loop = c->loop;
+  return SB_OK;
+}
+
+// Commits a verified checkpoint (the bulk sections are already on the device).
+int apply(sb_ctx* c, const StateImage& s) {
+  c->p = s.p;
+  derive(c);
+  c->confidence_threshold = s.confidence_threshold;
+  c->log_unstable_slam = s.log_unstable_slam;
+  c->timestamp = s.timestamp;
+  c->trackLoss = s.trackLoss;
+  memcpy(c->currentPose, s.currentPose, 128); memcpy(c->lastPose, s.lastPose, 128);
+  memcpy(c->currentPose_old, s.currentPose_old, 128); memcpy(c->currentPose_new, s.currentPose_new, 128);
+  memcpy(c->lastIncrement, s.lastIncrement, 128); memcpy(c->lastPose_old, s.lastPose_old, 128);
+  memcpy(c->stats, s.stats, sizeof(c->stats));
+  c->cur_has_semantics = s.cur_has_semantics != 0; c->last_has_semantics = s.last_has_semantics != 0;
+  c->close_loops = s.close_loops != 0;
+  c->loop = s.loop;
+  c->n_host = s.n_live; c->n_holes = 0; c->lazy_update = false; c->n_upper = s.n_live;
+  c->prepped_for_update = false;
+  c->map_timestamp = s.map_timestamp; c->pose_ref_end = s.pose_ref_end;
+  c->n_updated = s.n_updated; c->n_new = s.n_new;
+  c->origin_i = s.origin_i; c->origin_j = s.origin_j;
+  c->extraction = s.extraction;
+  c->tiles.clear();
+  for (const auto& t : s.tiles) c->tiles[t.first] = t.second;
+  c->n_slots = s.n_slots;
+  c->tiles_pending = s.tiles_pending != 0;
+  c->h_poses.assign((size_t)kMaxPoses * 16, 0.0f);
+  for (uint32_t t = 0; t < kMaxPoses; ++t)
+    for (int i = 0; i < 4; ++i) c->h_poses[16 * (size_t)t + 5 * i] = 1.0f;
+  c->h_poses_inv = c->h_poses;
+  memcpy(c->h_poses.data(), s.poses.data(), s.poses.size() * 4);
+  memcpy(c->h_poses_inv.data(), s.poses_inv.data(), s.poses_inv.size() * 4);
+  SB_CUDA(c, cudaMemcpyAsync(c->poses, c->h_poses.data(), (size_t)kMaxPoses * 64, cudaMemcpyHostToDevice, c->stream));
+  SB_CUDA(c, cudaMemcpyAsync(c->poses_inv, c->h_poses_inv.data(), (size_t)kMaxPoses * 64, cudaMemcpyHostToDevice,
+                             c->stream));
+  c->host->result = s.result;
+  SB_CUDA(c, cudaMemcpyAsync(c->res, &c->host->result, sizeof(ResultBlock), cudaMemcpyHostToDevice, c->stream));
+  if (s.n_slots)
+    SB_CUDA(c, cudaMemcpyAsync(c->d_tile_rec, s.tile_rec.data(), (size_t)s.n_slots * sizeof(uint2), cudaMemcpyHostToDevice,
+                               c->stream));
+  // scratch that a scan expects as the previous one left it: key images cleared by the pass that consumed them, group
+  // totals zero (a context that stopped mid-scan may not hold these; a loaded one does)
+  const size_t Pm = (size_t)c->kp.Wm * c->kp.Hm, Pk = preprocess_key_elems(c->kp.W, c->kp.H);
+  SB_CUDA(c, cudaMemsetAsync(c->key_old, 0xff, Pm * 8 * 3, c->stream));
+  for (int i = 0; i < 2; ++i) SB_CUDA(c, cudaMemsetAsync(c->prep.img[i], 0xff, Pk * 8, c->stream));
+  SB_CUDA(c, cudaMemsetAsync(c->group_counts, 0, kGroupCounts * 4, c->stream));
+  c->memo.clear();
+  c->map_version += 1;
+  SB_CUDA(c, cudaStreamSynchronize(c->stream));  // the copies read host vectors of `s` and members of the context
+  return SB_OK;
+}
+
+// Serialises everything but the bulk data; returns the offsets of the three bulk payloads and the total size.
+void layout(sb_ctx* c, const StateImage& s, Writer& head, std::vector<DevSection>& dev, uint64_t data_off[3],
+            uint64_t* total) {
+  Writer w;
+  write_host_sections(w, s);
+  dev = dev_sections(c, s.n_live, s.pool_end);
+  Writer hdr;
+  write_header(hdr, s, 0);
+  uint64_t off = hdr.b.size() + w.b.size();
+  for (int i = 0; i < 3; ++i) {
+    data_off[i] = off + 16;
+    off += 16 + dev[i].bytes();
+  }
+  *total = off + 8;
+  head.b.clear();
+  write_header(head, s, *total);
+  head.bytes(w.b.data(), w.b.size());
+}
+
+int state_check(sb_ctx* c) {
+  if (c->comm_on || c->comm_cb)
+    return fail(c, SB_ERR_STATE, "checkpoints are not available while a multi-GPU exchange is set up");
+  return SB_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int sb_state_size(sb_ctx* c, uint64_t* bytes) {
+  if (!c || !bytes) return fail(c, SB_ERR_INVALID, "state_size: null argument");
+  int r;
+  if ((r = state_check(c))) return r;
+  cudaSetDevice(c->device);
+  StateImage s;
+  if ((r = capture(c, s))) return r;
+  Writer head;
+  std::vector<DevSection> dev;
+  uint64_t off[3];
+  layout(c, s, head, dev, off, bytes);
+  return SB_OK;
+}
+
+int sb_state_save(sb_ctx* c, void* dst, uint64_t cap, uint64_t* written) {
+  if (!c || !dst) return fail(c, SB_ERR_INVALID, "state_save: null argument");
+  int r;
+  if ((r = state_check(c))) return r;
+  cudaSetDevice(c->device);
+  StateImage s;
+  if ((r = capture(c, s))) return r;
+  Writer head;
+  std::vector<DevSection> dev;
+  uint64_t off[3], total = 0;
+  layout(c, s, head, dev, off, &total);
+  if (written) *written = total;
+  if (cap < total) return fail(c, SB_ERR_INVALID, "state_save: buffer smaller than sb_state_size");
+  if ((r = discard_prefetch(c))) return r;
+  if ((r = state_staging(c))) return r;
+  uint8_t* out = static_cast<uint8_t*>(dst);
+  memcpy(out, head.b.data(), head.b.size());
+  uint64_t digest = host_digest(out, 0, head.b.size());
+  for (int i = 0; i < 3; ++i) {  // section headers of the bulk data
+    const uint32_t id = dev[i].id, zero = 0;
+    const uint64_t len = dev[i].bytes();
+    memcpy(out + off[i] - 16, &id, 4); memcpy(out + off[i] - 12, &zero, 4); memcpy(out + off[i] - 8, &len, 8);
+    digest += host_digest(out, off[i] - 16, 16);
+  }
+  SB_CUDA(c, cudaMemsetAsync(c->state_acc, 0, 8, c->stream));
+  c->lb_gen = (c->lb_gen + 1) & 0x3fffffffu;
+  if (c->lb_gen == 0) c->lb_gen = 1;
+  launch_state_pack(L_(c), c->A, c->live, c->n_host, c->T.p0, s.n_live, c->lb_desc, c->lb_ticket, c->lb_gen, off[0] / 8,
+                    c->state_acc);
+  digest_ranges(c, dev[1], off[1]);
+  digest_ranges(c, dev[2], off[2]);
+  SB_CUDA(c, cudaGetLastError());
+  for (int i = 0; i < 3; ++i)
+    if ((r = copy_out(c, dev[i].ranges, out + off[i]))) return r;
+  unsigned long long dd = 0;
+  SB_CUDA(c, cudaMemcpyAsync(&c->host->sums[0], c->state_acc, 8, cudaMemcpyDeviceToHost, c->stream));
+  SB_CUDA(c, cudaStreamSynchronize(c->stream));
+  memcpy(&dd, &c->host->sums[0], 8);
+  digest += dd;
+  memcpy(out + total - 8, &digest, 8);
+  return SB_OK;
+}
+
+int sb_state_load(sb_ctx* c, const void* src, uint64_t n) {
+  if (!c || (!src && n)) return fail(c, SB_ERR_INVALID, "state_load: null argument");
+  int r;
+  if ((r = state_check(c))) return r;
+  StateImage s;
+  Reader rd{static_cast<const uint8_t*>(src), (size_t)n};
+  if (const char* why = read_host(rd, c, s)) return fail(c, SB_ERR_INVALID, std::string("state_load: ") + why);
+  cudaSetDevice(c->device);
+  std::vector<DevSection> dev = dev_sections(c, s.n_live, s.pool_end);
+  uint64_t off[3];
+  for (int i = 0; i < 3; ++i) {
+    const uint64_t len = read_open(rd, dev[i].id);
+    off[i] = rd.off;
+    if (!rd.ok || len != dev[i].bytes()) return fail(c, SB_ERR_INVALID, "state_load: malformed bulk section");
+    rd.off += len;
+  }
+  if (rd.n - rd.off != 8) return fail(c, SB_ERR_INVALID, "state_load: checkpoint size does not match its sections");
+  // ---- the header is sound: from here on the context changes ----
+  if ((r = discard_prefetch(c))) return r;
+  if ((r = state_staging(c))) return r;
+  const uint8_t* in = static_cast<const uint8_t*>(src);
+  uint64_t digest = host_digest(in, 0, off[0]);
+  for (int i = 1; i < 3; ++i) digest += host_digest(in, off[i] - 16, 16);
+  SB_CUDA(c, cudaMemsetAsync(c->state_acc, 0, 8, c->stream));
+  for (int i = 0; i < 3; ++i)
+    if ((r = copy_in(c, dev[i].ranges, in + off[i]))) return r;
+  launch_state_unpack(L_(c), c->T.p0, s.n_live, c->A, c->live, off[0] / 8, c->state_acc);
+  digest_ranges(c, dev[1], off[1]);
+  digest_ranges(c, dev[2], off[2]);
+  SB_CUDA(c, cudaGetLastError());
+  SB_CUDA(c, cudaMemcpyAsync(&c->host->sums[0], c->state_acc, 8, cudaMemcpyDeviceToHost, c->stream));
+  SB_CUDA(c, cudaStreamSynchronize(c->stream));
+  unsigned long long dd = 0;
+  memcpy(&dd, &c->host->sums[0], 8);
+  digest += dd;
+  uint64_t stored;
+  memcpy(&stored, in + n - 8, 8);
+  if (digest != stored) {
+    // bulk sections are already overwritten: never leave a half-loaded context behind
+    if ((r = reset_state(c))) return r;
+    return fail(c, SB_ERR_INVALID, "state_load: checkpoint digest mismatch (corrupted data); the context was reset");
+  }
+  return apply(c, s);
 }
 
 }  // extern "C"

@@ -157,7 +157,8 @@ cudaError_t dev_alloc(DevPtr<T>& p, size_t bytes) {
 enum KernelId {
   K_FILL = 0, K_PROJECT_SCATTER, K_PREPROCESS_TILE, K_ICP_JACOBIAN, K_GN_INIT,
   K_ICP_FUSED, K_POSE_PRODUCTS, K_RENDER_SCATTER, K_RENDER_RESOLVE, K_INDEX_SCATTER, K_RADIUS, K_UPDATE_SURFELS,
-  K_GEN_SURFELS, K_EXTRACT_FLAGS, K_COMPACT_SCATTER, K_AOS_TO_SOA, K_SOA_TO_AOS, K_ICP_POST, K_COUNT
+  K_GEN_SURFELS, K_EXTRACT_FLAGS, K_COMPACT_SCATTER, K_AOS_TO_SOA, K_SOA_TO_AOS, K_ICP_POST, K_STATE_PACK,
+  K_STATE_UNPACK, K_STATE_DIGEST, K_COUNT
 };
 const char* kernel_name(int id);
 
@@ -306,5 +307,29 @@ void launch_extract_to_pool(const Launch& L, SurfelPlanes map, const uint32_t* n
                             uint32_t tile_cap);
 void launch_aos_to_soa(const Launch& L, const sb_surfel* aos, SurfelPlanes s, uint32_t offset, uint32_t n);
 void launch_soa_to_aos(const Launch& L, SurfelPlanes s, sb_surfel* aos, uint32_t n);
+
+// ---- checkpoint digest (sb_state_save / sb_state_load) ----
+// The digest of a checkpoint is the sum mod 2^64 of state_word_hash(i, w) over its little-endian 64-bit words w at word
+// offset i. Keyed by position, it changes when words move; being a sum, the blocks of a kernel and the host's part combine
+// into the same value whatever order they are added in.
+__host__ __device__ inline uint64_t state_mix64(uint64_t x) {  // splitmix64 finaliser
+  x ^= x >> 30; x *= 0xbf58476d1ce4e5b9ull;
+  x ^= x >> 27; x *= 0x94d049bb133111ebull;
+  x ^= x >> 31;
+  return x;
+}
+__host__ __device__ inline uint64_t state_word_hash(uint64_t pos, uint64_t w) {
+  return state_mix64(w ^ state_mix64(pos + 0x9e3779b97f4a7c15ull));
+}
+// The live surfels of map slots [0, n_phys), in order, into `flat` as four lanes of pitch n_live (p0[n_live], p1[...], ...),
+// with their digest at blob word offset word_base added to *acc. Single pass: decoupled look-back (sb_map.cu).
+void launch_state_pack(const Launch& L, SurfelPlanes map, const uint8_t* live, uint32_t n_phys, float4* flat,
+                       uint32_t n_live, unsigned long long* desc, uint32_t* ticket, uint32_t gen, uint64_t word_base,
+                       unsigned long long* acc);
+// the reverse into a dense map: flat lanes of pitch n -> map slots [0, n), liveness set, digest added to *acc
+void launch_state_unpack(const Launch& L, const float4* flat, uint32_t n, SurfelPlanes map, uint8_t* live,
+                         uint64_t word_base, unsigned long long* acc);
+// digest of n_words device words at blob word offset word_base, added to *acc
+void launch_state_digest(const Launch& L, const void* words, uint64_t n_words, uint64_t word_base, unsigned long long* acc);
 
 }  // namespace sb

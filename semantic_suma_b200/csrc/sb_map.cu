@@ -26,7 +26,8 @@ const char* kernel_name(int id) {
   static const char* names[K_COUNT] = {"fill_u64", "project_scatter", "preprocess_tile",
                                        "icp_jacobian", "gn_init", "icp_fused", "pose_products", "render_scatter",
                                        "render_resolve", "index_scatter", "radius", "update_surfels", "gen_surfels",
-                                       "extract_flags", "compact_scatter", "aos_to_soa", "soa_to_aos", "icp_post"};
+                                       "extract_flags", "compact_scatter", "aos_to_soa", "soa_to_aos", "icp_post",
+                                       "state_pack", "state_unpack", "state_digest"};
   return (id >= 0 && id < K_COUNT) ? names[id] : "?";
 }
 
@@ -1405,6 +1406,114 @@ void launch_soa_to_aos(const Launch& L, SurfelPlanes s, sb_surfel* aos, uint32_t
   {
     ScopedKernel sk(L, K_SOA_TO_AOS);
     k_soa_to_aos<<<(n + kThreads - 1) / kThreads, kThreads, 0, L.stream>>>(s, reinterpret_cast<float4*>(aos), n);
+  }
+}
+
+// ---- checkpoints (sb_state_save / sb_state_load): ordered gather of the live map, scatter back, position-keyed digest ----
+__device__ __forceinline__ uint64_t lane_digest(float4 v, uint64_t pos) {  // the two 64-bit words of one 16-byte lane
+  const uint64_t w0 = ((uint64_t)__float_as_uint(v.y) << 32) | __float_as_uint(v.x);
+  const uint64_t w1 = ((uint64_t)__float_as_uint(v.w) << 32) | __float_as_uint(v.z);
+  return state_word_hash(pos, w0) + state_word_hash(pos + 1, w1);
+}
+
+// one atomic per block: the block's sum (exact mod 2^64, so the order of the blocks' additions does not matter)
+__device__ __forceinline__ void block_digest_add(uint64_t h, unsigned long long* acc) {
+  __shared__ uint64_t s_h[kThreads / 32];
+  for (int o = 16; o > 0; o >>= 1) h += __shfl_xor_sync(0xffffffffu, h, o);
+  if ((threadIdx.x & 31) == 0) s_h[threadIdx.x >> 5] = h;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    uint64_t t = 0;
+    for (int w = 0; w < kThreads / 32; ++w) t += s_h[w];
+    atomicAdd(acc, (unsigned long long)t);
+  }
+}
+
+__global__ void __launch_bounds__(kThreads) k_state_pack(SurfelPlanes s, const uint8_t* __restrict__ live, uint32_t n_phys,
+                                                        float4* __restrict__ flat, uint32_t n_live, Lookback lb,
+                                                        uint64_t word_base, unsigned long long* acc) {
+  const uint32_t vb = block_ticket(lb);
+  const uint32_t k = vb * blockDim.x + threadIdx.x;
+  const bool kept = k < n_phys && live[k] != 0;
+  float4 v0, v1, v2, v3;
+  v0 = v1 = v2 = v3 = make_float4(0.f, 0.f, 0.f, 0.f);
+  if (kept) {
+    v0 = s.p0[k]; v1 = s.p1[k]; v2 = s.p2[k]; v3 = s.p3[k];
+  }
+  uint32_t block_count;
+  const uint32_t rank = block_rank<kThreads>(kept, block_count);
+  const uint32_t excl = lookback_exclusive(lb, vb, block_count);
+  uint64_t h = 0;
+  if (kept) {
+    const uint32_t d = excl + rank;  // < n_live: the host counted the live slots
+    const float4 v[4] = {v0, v1, v2, v3};
+#pragma unroll
+    for (int l = 0; l < 4; ++l) {
+      const size_t i = (size_t)l * n_live + d;
+      flat[i] = v[l];
+      h += lane_digest(v[l], word_base + 2 * i);
+    }
+  }
+  block_digest_add(h, acc);
+  if (vb == gridDim.x - 1 && threadIdx.x == 0) *lb.ticket = 0;
+}
+
+__global__ void __launch_bounds__(kThreads) k_state_unpack(const float4* __restrict__ flat, uint32_t n, SurfelPlanes s,
+                                                          uint8_t* __restrict__ live, uint64_t word_base,
+                                                          unsigned long long* acc) {
+  const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  uint64_t h = 0;
+  if (k < n) {
+    float4* dst[4] = {s.p0, s.p1, s.p2, s.p3};
+#pragma unroll
+    for (int l = 0; l < 4; ++l) {
+      const size_t i = (size_t)l * n + k;
+      const float4 v = flat[i];
+      dst[l][k] = v;
+      h += lane_digest(v, word_base + 2 * i);
+    }
+    live[k] = 1;
+  }
+  block_digest_add(h, acc);
+}
+
+__global__ void __launch_bounds__(kThreads) k_state_digest(const unsigned long long* __restrict__ w, uint64_t n,
+                                                          uint64_t word_base, unsigned long long* acc) {
+  uint64_t h = 0;
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x)
+    h += state_word_hash(word_base + i, w[i]);
+  block_digest_add(h, acc);
+}
+
+void launch_state_pack(const Launch& L, SurfelPlanes map, const uint8_t* live, uint32_t n_phys, float4* flat,
+                       uint32_t n_live, unsigned long long* desc, uint32_t* ticket, uint32_t gen, uint64_t word_base,
+                       unsigned long long* acc) {
+  if (n_phys == 0) return;
+  Lookback lb{desc, ticket, gen};
+  {
+    ScopedKernel sk(L, K_STATE_PACK);
+    k_state_pack<<<(n_phys + kThreads - 1) / kThreads, kThreads, 0, L.stream>>>(map, live, n_phys, flat, n_live, lb,
+                                                                               word_base, acc);
+  }
+}
+
+void launch_state_unpack(const Launch& L, const float4* flat, uint32_t n, SurfelPlanes map, uint8_t* live,
+                         uint64_t word_base, unsigned long long* acc) {
+  if (n == 0) return;
+  {
+    ScopedKernel sk(L, K_STATE_UNPACK);
+    k_state_unpack<<<(n + kThreads - 1) / kThreads, kThreads, 0, L.stream>>>(flat, n, map, live, word_base, acc);
+  }
+}
+
+void launch_state_digest(const Launch& L, const void* words, uint64_t n_words, uint64_t word_base, unsigned long long* acc) {
+  if (n_words == 0) return;
+  uint64_t blocks = (n_words + kThreads - 1) / kThreads;
+  if (blocks > 1024) blocks = 1024;
+  {
+    ScopedKernel sk(L, K_STATE_DIGEST);
+    k_state_digest<<<(unsigned)blocks, kThreads, 0, L.stream>>>(static_cast<const unsigned long long*>(words), n_words,
+                                                                 word_base, acc);
   }
 }
 

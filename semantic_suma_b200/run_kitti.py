@@ -9,6 +9,11 @@
     python -m semantic_suma_b200.run_kitti <seq> [--out poses_out.txt] [--semantic] [--max-scans N] [--width 2048]
     python -m semantic_suma_b200.run_kitti --make-synthetic <dir> --scans 50     # writes such a directory
 
+Long runs can be checkpointed and resumed (sb_state_save / sb_state_load): --save-state PATH writes the library's state
+to PATH and the trajectory so far to PATH.poses.npy, after every --save-every N scans and at the end of the run;
+--resume PATH continues at the scan after the saved one. The pose file of a resumed run is byte-identical to the one of
+an uninterrupted run.
+
 The engine is the CUDA library (an H100 is required); tests inject another engine through `make_engine` to check the
 file plumbing without a GPU.
 """
@@ -33,18 +38,53 @@ def _cuda_engine(params):
     return api.SurfelMapping(params)
 
 
-def run_sequence(seq_dir, params, make_engine=None, semantic=False, max_scans=None, on_scan=None):
-    """-> dict(poses=[4x4 float64 in the velodyne frame], seconds, scans). `make_engine(params)` must return an object
-    with processScan(points4, labels, probs) and getCurrentPose() -- the SurfelMapping surface."""
+def trajectory_path(state_path):
+    return state_path + ".poses.npy"
+
+
+def write_checkpoint(engine, state_path, poses):
+    """the engine's state to `state_path`, the poses so far beside it; each file is replaced only once it is complete,
+    the trajectory last, so that an interrupted save leaves the previous checkpoint readable"""
+    blob = engine.save_state()
+    tmp = state_path + ".tmp"
+    with open(tmp, "wb") as f:
+        f.write(blob)
+    os.replace(tmp, state_path)
+    tmp = trajectory_path(state_path) + ".tmp.npy"
+    np.save(tmp, np.asarray(poses, np.float64).reshape(-1, 4, 4))
+    os.replace(tmp, trajectory_path(state_path))
+
+
+def read_checkpoint(engine, state_path):
+    """loads `state_path` into the engine; -> the poses saved with it (one per scan already processed)"""
+    with open(state_path, "rb") as f:
+        engine.load_state(f.read())
+    poses = [p.copy() for p in np.load(trajectory_path(state_path))]
+    if engine.timestamp() != len(poses):
+        raise ValueError("%s holds %d scans but its trajectory %d poses" % (state_path, engine.timestamp(), len(poses)))
+    return poses
+
+
+def run_sequence(seq_dir, params, make_engine=None, semantic=False, max_scans=None, on_scan=None, save_state=None,
+                 save_every=None, resume=None):
+    """-> dict(poses=[4x4 float64 in the velodyne frame, from scan 0], seconds, scans processed by this call).
+    `make_engine(params)` must return an object with processScan(points4, labels, probs) and getCurrentPose() -- the
+    SurfelMapping surface -- and, for save_state / resume, save_state(), load_state(bytes) and timestamp().
+    resume: a checkpoint written by save_state; the run continues at the scan after it."""
     files = list_scans(seq_dir)
     if max_scans is not None:
         files = files[:max_scans]
     if not files:
         raise FileNotFoundError("no scans under %s/velodyne" % seq_dir)
     engine = (make_engine or _cuda_engine)(params)
-    poses = []
+    poses = read_checkpoint(engine, resume) if resume else []
+    first = len(poses)
+    if first > len(files):
+        raise ValueError("%s is past the end of the sequence (%d scans)" % (resume, len(files)))
     t0 = time.time()
     for i, f in enumerate(files):
+        if i < first:
+            continue
         pts, _ = kitti.read_scan(f)
         labels = probs = None
         if semantic:
@@ -54,7 +94,11 @@ def run_sequence(seq_dir, params, make_engine=None, semantic=False, max_scans=No
         poses.append(np.asarray(engine.getCurrentPose(), np.float64).copy())
         if on_scan:
             on_scan(i, poses[-1])
-    return {"poses": poses, "seconds": time.time() - t0, "scans": len(files)}
+        if save_state and save_every and (i + 1) % save_every == 0 and i + 1 < len(files):
+            write_checkpoint(engine, save_state, poses)
+    if save_state:
+        write_checkpoint(engine, save_state, poses)
+    return {"poses": poses, "seconds": time.time() - t0, "scans": len(files) - first}
 
 
 def evaluate_against_ground_truth(seq_dir, poses_velo):
@@ -99,7 +143,7 @@ def make_synthetic_sequence(seq_dir, n_scans, width=2048, height=64, semantic=Fa
     return seq_dir
 
 
-def main(argv=None):
+def main(argv=None, make_engine=None):
     ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
     ap.add_argument("seq", nargs="?")
     ap.add_argument("--out", default=None, help="pose file to write (KITTI format; camera frame if calib.txt has Tr)")
@@ -108,7 +152,13 @@ def main(argv=None):
     ap.add_argument("--width", type=int, default=2048)
     ap.add_argument("--make-synthetic", default=None, metavar="DIR")
     ap.add_argument("--scans", type=int, default=50)
+    ap.add_argument("--save-state", default=None, metavar="PATH",
+                    help="checkpoint file (and PATH.poses.npy): written at the end and every --save-every scans")
+    ap.add_argument("--save-every", type=int, default=None, metavar="N")
+    ap.add_argument("--resume", default=None, metavar="PATH", help="continue from a --save-state checkpoint")
     args = ap.parse_args(argv)
+    if args.save_every is not None and (args.save_every <= 0 or not args.save_state):
+        ap.error("--save-every needs --save-state and N > 0")
     if args.make_synthetic:
         make_synthetic_sequence(args.make_synthetic, args.scans, width=args.width, semantic=args.semantic)
         print("wrote", args.make_synthetic)
@@ -118,13 +168,14 @@ def main(argv=None):
         ap.error("need a sequence directory")
     from . import api
     params = api.default_params(data_width=args.width, model_width=args.width)
-    res = run_sequence(args.seq, params, semantic=args.semantic, max_scans=args.max_scans)
+    res = run_sequence(args.seq, params, make_engine=make_engine, semantic=args.semantic, max_scans=args.max_scans,
+                       save_state=args.save_state, save_every=args.save_every, resume=args.resume)
     calib_file = os.path.join(args.seq, "calib.txt")
     Tr = kitti.read_calibration(calib_file).get("Tr") if os.path.exists(calib_file) else None
     if args.out:
         kitti.save_poses(args.out, res["poses"], Tr=Tr)
     report = {"scans": res["scans"], "seconds": round(res["seconds"], 3),
-              "scans_per_sec_incl_file_io": round(res["scans"] / res["seconds"], 2),
+              "scans_per_sec_incl_file_io": round(res["scans"] / res["seconds"], 2) if res["seconds"] > 0 else None,
               "odometry": evaluate_against_ground_truth(args.seq, res["poses"])}
     print(json.dumps(report))
     return 0
