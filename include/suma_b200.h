@@ -91,6 +91,7 @@ int sb_default_params(sb_params* p);                               /* config/def
 /* sb_create and sb_set_params return SB_ERR_INVALID (reason on stderr / in sb_last_error) for:
  *  - image sizes <= 0, more than 2^24 data pixels, or a data width of 1 (the preprocessing stencils reach two columns
  *    around the azimuth seam, which one column cannot provide);
+ *  - a model image side over 65536 pixels (the render pass packs a quad's pixel box origin in 16 bits per axis);
  *  - depth ranges with max <= min;
  *  - parameters whose exact ICP sums could leave the int64 range: data pixels x (max(max_depth, model_max_depth) + 25 m)^2
  *    x 2^30 > 2^63 - 1. The 25 m allow for the translation of the pose. 128x4096 at 75 m is accepted; the largest image

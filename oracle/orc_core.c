@@ -60,6 +60,8 @@ const char* orc_check_params(const orc_params* p) {
   if (p->data_width <= 0 || p->data_height <= 0 || p->model_width <= 0 || p->model_height <= 0) return "image size <= 0";
   if ((size_t)p->data_width * p->data_height > (1u << 24)) return "more than 2^24 data pixels";
   if (p->data_width < 2) return "data width < 2";
+  if (p->model_width > 65536 || p->model_height > 65536)
+    return "model image side > 65536 (the render pass packs pixel boxes in 16 bits)";
   if (!(p->max_depth > p->min_depth) || !(p->model_max_depth > p->model_min_depth)) return "max depth <= min depth";
   const double range = (p->max_depth > p->model_max_depth ? p->max_depth : p->model_max_depth) + 25.0;
   if ((double)p->data_width * p->data_height * range * range * 1073741824.0 > 9223372036854775807.0)

@@ -1228,6 +1228,9 @@ static const char* check_params(const sb_params* p) {
   if ((size_t)p->data_width * p->data_height > (1u << 24)) return "more than 2^24 data pixels";
   // the stencils of preprocessing reach 2 columns around the azimuth seam; one column cannot wrap onto itself twice
   if (p->data_width < 2) return "data width < 2";
+  // k_render_scatter packs a small quad's pixel box origin as i0 | j0 << 16 (QuadStore::box)
+  if (p->model_width > 65536 || p->model_height > 65536)
+    return "model image side > 65536 (the render pass packs pixel boxes in 16 bits)";
   if (!(p->max_depth > p->min_depth) || !(p->model_max_depth > p->model_min_depth)) return "max depth <= min depth";
   // Q33.30 head-room of the exact ICP sums: no int64 sum may wrap (DESIGN.md section 2)
   const double range = (p->max_depth > p->model_max_depth ? p->max_depth : p->model_max_depth) + kIcpPoseMargin;

@@ -566,8 +566,8 @@ __global__ void __launch_bounds__(kRenderThreads, kMinBlocks) k_render_scatter(K
       // phase 2
       for (int i0q = 0; i0q < qn; i0q += 32 * kFragBatch) {
         // per fragment only the queue entry, the pixel and the fetched key stay live; the key image is chosen again from
-        // the surfel class when it is used. The pixel index fits 32 bits: Q.box holds i0 and j0 in 16 bits each, which
-        // already limits the model image to 65536 x 65536 pixels, so the index is at most 2^32 - 1.
+        // the surfel class when it is used. The pixel index fits 32 bits: Q.box holds i0 and j0 in 16 bits each, and
+        // sb_create refuses model images with a side over 65536 (check_params), so the index is at most 2^32 - 1.
         uint32_t ent[kFragBatch], pixs[kFragBatch];
         unsigned long long cur[kFragBatch];
 #pragma unroll

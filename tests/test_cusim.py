@@ -55,6 +55,13 @@ def test_map_update_on_an_image_under_256_pixels():
     assert _child(["tests/test_gpu_shapes.py"], "test_map_updates_on_an_image_under_256_pixels") == 1
 
 
+def test_render_edges_on_the_cpu_executor():
+    """the render pass at the switch points of its fast paths (small / large quads, corner span, azimuth seam, degenerate
+    and crossed quads, the tie rule, depth ties, z clip, block loads, a 65536-wide model image) against the exact reference
+    rasteriser and the oracle, and the refusal of model sides over 65536 (tests/test_gpu_render_edges.py)"""
+    assert _child(["tests/test_gpu_render_edges.py"], "test_") == 15
+
+
 def test_submap_paging_on_the_cpu_executor():
     """several tiles extracted per update, a tile over the 500 000-surfel extract cap and paging an empty map, each against
     the oracle (tests/test_gpu_paging.py; the pool exhaustion case runs in the full tier)"""
