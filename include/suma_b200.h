@@ -169,6 +169,26 @@ int sb_map_set_pose(sb_ctx* ctx, uint32_t t, const float pose[16]);
 int sb_map_update_debug(sb_ctx* ctx, uint32_t* index_map, float* radius_map4, uint8_t* integrated,
                         uint32_t* n_updated, uint32_t* n_new);
 int sb_map_submap_origin(sb_ctx* ctx, int32_t* i, int32_t* j, uint32_t* pending);
+/* ---- managed submap tile cache (no counterpart in the reference, whose submapCache_ is host RAM without a bound) ----
+ * By default the tiles that leave the active window go into an append-only HBM pool of 16 M surfels: every extraction
+ * takes new pool space and a record slot (16384 in all), and a surfel that finds the pool full is dropped (stats[12]).
+ * sb_set_tile_cache makes the cache of this context managed: abandoned pool ranges are reclaimed on the device, cold
+ * tiles move to pinned host memory and come back from it, and record slots are reused, so that a surfel is dropped only
+ * when both tiers are full (counted in stats[12] with the same message). The map's bits do not depend on the tier a tile
+ * lived in. pool_surfels: the HBM share, 500 000 <= pool_surfels <= 16 M; host_surfels: surfels that may live in host
+ * memory (UINT64_MAX = no bound, as in the reference). Valid while the cache is empty (after sb_create / sb_reset,
+ * before the first extraction): SB_ERR_STATE otherwise. Kept across sb_reset; saved and restored by sb_state_save /
+ * sb_state_load (a checkpoint of a default context makes the loading context default again). */
+int sb_set_tile_cache(sb_ctx* ctx, uint32_t pool_surfels, uint64_t host_surfels);
+typedef struct sb_tile_cache_info {
+  uint32_t managed, tiles_in_pool, tiles_on_host, pad;
+  uint64_t pool_capacity, pool_used, pool_referenced; /* surfels: capacity, used range, held by cached tiles */
+  uint64_t host_capacity, host_used;
+  uint64_t reclaims, reclaim_moved, evictions, host_fills, dropped; /* pool compactions and the surfels they moved,
+                                                                       tiles moved to / re-inserted from the host,
+                                                                       surfels dropped (stats[12]) */
+} sb_tile_cache_info;
+int sb_get_tile_cache_info(sb_ctx* ctx, sb_tile_cache_info* out);
 
 /* ---- SurfelMapping::processScan, SurfelMapping.cpp:175-210 (loop closure off) ---------------------------------- */
 int sb_process_scan(sb_ctx* ctx, const float* pts4, const float* labels, const float* probs, uint32_t n,
@@ -227,7 +247,7 @@ int sb_slam_frame(sb_ctx* ctx, int which, sb_frame** out); /* getCurrentFrame / 
  * no counterpart -- the stages overlap on the stream -- so their slots [8] [9] [10] carry the host-side split of the
  * call: enqueue / wait for the device / bookkeeping after the wait;
  * [12] surfels dropped because the HBM cache of extracted submap tiles (16 M surfels) was full -- the reference's
- * host-side submapCache_ is unbounded; sb_last_error carries the message */
+ * host-side submapCache_ is unbounded; sb_last_error carries the message (with sb_set_tile_cache: both tiers full) */
 int sb_get_statistics(sb_ctx* ctx, double stats[16]);
 
 /* ---- checkpoint / resume (no counterpart in the reference: its Posegraph::save/load are empty stubs) --------------

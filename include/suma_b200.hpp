@@ -400,6 +400,16 @@ class SurfelMap {
   template <class ColorMap>
   void setColorMap(const ColorMap&) {}
   void reset() { check(sb_reset(ctx_->get()), ctx_->get(), "SurfelMap::reset"); }
+  /** managed submap tile cache (sb_set_tile_cache; no counterpart in the reference): host_surfels = UINT64_MAX for no
+   * bound. Only while the cache is empty (after construction or reset). */
+  void setTileCache(uint32_t pool_surfels, uint64_t host_surfels) {
+    check(sb_set_tile_cache(ctx_->get(), pool_surfels, host_surfels), ctx_->get(), "SurfelMap::setTileCache");
+  }
+  sb_tile_cache_info tileCacheInfo() const {
+    sb_tile_cache_info info;
+    check(sb_get_tile_cache_info(ctx_->get(), &info), ctx_->get(), "SurfelMap::tileCacheInfo");
+    return info;
+  }
   void update(const Matrix4f& pose, Frame& frame) {
     check(sb_map_update(ctx_->get(), pose.m, frame.handle()), ctx_->get(), "SurfelMap::update");
   }
@@ -451,6 +461,9 @@ class SurfelMapping {
   explicit SurfelMapping(const ParameterList& params, int device = 0)
       : ctx_(std::make_shared<Context>(params, device)), map_(std::make_shared<SurfelMap>(ctx_)) {}
   void setParameters(const ParameterList& params) { ctx_->setParameters(params); }
+  /** managed submap tile cache: see SurfelMap::setTileCache */
+  void setTileCache(uint32_t pool_surfels, uint64_t host_surfels) { map_->setTileCache(pool_surfels, host_surfels); }
+  sb_tile_cache_info tileCacheInfo() const { return map_->tileCacheInfo(); }
   void reset() {
     check(sb_reset(ctx_->get()), ctx_->get(), "SurfelMapping::reset");
     trajectory_.clear();

@@ -39,6 +39,15 @@ class LoopEdge(C.Structure):  # sb_loop_edge
     _fields_ = [("from_", C.c_int32), ("to", C.c_int32), ("rel_pose", C.c_double * 16)]
 
 
+class TileCacheInfo(C.Structure):  # sb_tile_cache_info
+    _fields_ = [(n, C.c_uint32) for n in ("managed", "tiles_in_pool", "tiles_on_host", "pad")] + \
+               [(n, C.c_uint64) for n in ("pool_capacity", "pool_used", "pool_referenced", "host_capacity", "host_used",
+                                          "reclaims", "reclaim_moved", "evictions", "host_fills", "dropped")]
+
+
+HOST_UNBOUNDED = 2**64 - 1  # sb_set_tile_cache: no bound on the host tier
+
+
 class Params(C.Structure):
     _fields_ = [
         ("data_width", C.c_int32), ("data_height", C.c_int32),
@@ -147,6 +156,7 @@ def lib(build_if_missing=True):
         "sb_profile_kernels": [],
         "sb_state_size": [vp, C.POINTER(C.c_uint64)], "sb_state_save": [vp, vp, C.c_uint64, C.POINTER(C.c_uint64)],
         "sb_state_load": [vp, vp, C.c_uint64],
+        "sb_set_tile_cache": [vp, u32, C.c_uint64], "sb_get_tile_cache_info": [vp, C.POINTER(TileCacheInfo)],
     }
     for name, args in sig.items():
         fn = getattr(L, name)
@@ -177,6 +187,7 @@ EXPORTED_SYMBOLS = [
     "sb_profile_enable", "sb_default_loop_params", "sb_set_loop_closure", "sb_get_loop_info", "sb_get_loop_edges",
     "sb_set_current_pose", "sb_integrate_loop_closures",
     "sb_profile_kernels", "sb_profile_name", "sb_profile_collect", "sb_state_size", "sb_state_save", "sb_state_load",
+    "sb_set_tile_cache", "sb_get_tile_cache_info",
 ]
 
 
@@ -266,6 +277,19 @@ class Context:
         p = Params()
         self.check(lib().sb_get_params(self.h, C.byref(p)), "get_params")
         return p
+
+    def set_tile_cache(self, pool_surfels, host_surfels=None):
+        """Managed submap tile cache (sb_set_tile_cache): pool_surfels in HBM (500 000 .. 16 M), host_surfels in pinned
+        host memory (None or inf: no bound). Only while the cache is empty: after creation or reset."""
+        if host_surfels is None or host_surfels == float("inf"):
+            host_surfels = HOST_UNBOUNDED
+        self.check(lib().sb_set_tile_cache(self.h, int(pool_surfels), int(host_surfels)), "set_tile_cache")
+
+    def tile_cache_info(self):
+        """counters of the submap tile cache (sb_get_tile_cache_info) as a dict"""
+        o = TileCacheInfo()
+        self.check(lib().sb_get_tile_cache_info(self.h, C.byref(o)), "get_tile_cache_info")
+        return {n: int(getattr(o, n)) for n, _ in TileCacheInfo._fields_ if n != "pad"}
 
     def set_params(self, params):
         self.check(lib().sb_set_params(self.h, C.byref(params)), "set_params")
@@ -535,6 +559,12 @@ class SurfelMap:
         lib().sb_map_submap_origin(self.ctx.h, C.byref(i), C.byref(j), C.byref(p))
         return i.value, j.value, p.value
 
+    def setTileCache(self, pool_surfels, host_surfels=None):
+        self.ctx.set_tile_cache(pool_surfels, host_surfels)
+
+    def tile_cache_info(self):
+        return self.ctx.tile_cache_info()
+
     def reset(self):
         self.ctx.check(lib().sb_reset(self.ctx.h), "reset")
 
@@ -650,6 +680,13 @@ class SurfelMapping:
 
     def getLastModelFrame(self):
         return self._frame(3)
+
+    def setTileCache(self, pool_surfels, host_surfels=None):
+        """Managed submap tile cache: see Context.set_tile_cache"""
+        self.ctx.set_tile_cache(pool_surfels, host_surfels)
+
+    def tile_cache_info(self):
+        return self.ctx.tile_cache_info()
 
     def getStatistics(self):
         a = np.zeros(16)

@@ -33,6 +33,12 @@ struct DevTile {  // SubmapCache, SurfelMap.h:179-181 -- kept in HBM (tile pool)
   uint32_t base = 0, count = 0;
 };
 
+// A tile of the managed cache's host tier: its surfels as four lanes of pitch `count` in a pinned buffer of `cap` surfels
+struct HostTile {
+  uint32_t count = 0, cap = 0;
+  PinnedPtr<float4> buf;
+};
+
 struct sb_ctx {
   int device = 0;
   int sm_count = 132;
@@ -132,6 +138,19 @@ struct sb_ctx {
   DevPtr<uint2> d_tile_rec;       // {end in the pool, surfels of the tile} per extraction; slot s starts at the end of s - 1
   uint32_t n_slots = 0;
   bool tiles_pending = false;     // some records have not been read back yet
+  // managed tile cache (sb_set_tile_cache; DESIGN.md section 10): off by default, and then none of this is touched
+  struct TileCache {
+    bool managed = false;
+    uint32_t pool_cap = kTilePoolCap;  // HBM share (the pool allocation stays kTilePoolCap)
+    uint64_t host_cap = 0;             // surfels the host tier may hold
+    uint64_t pool_bound = 0;           // upper bound of the pool's used end that the host has without a read-back
+    uint64_t host_used = 0;
+    uint64_t reclaims = 0, reclaim_moved = 0, evictions = 0, host_fills = 0;
+    uint64_t dropped_retired = 0;      // drops counted on record slots that a reclaim has since renumbered
+    std::map<std::pair<int32_t, int32_t>, HostTile> host;  // host-resident tiles (never also in `tiles`)
+    std::multimap<uint32_t, PinnedPtr<float4>> spare;       // pinned buffers of replaced host tiles, by capacity
+    DevPtr<uint2> segs;                // move list of a reclaim
+  } tc;
 
   // Full-render memo: SurfelMapping re-renders the unchanged map at the unchanged pose at the start of the next scan
   // (SurfelMapping.cpp:351 after :803); identical arguments on an unmodified map reproduce identical images. The memo
@@ -279,6 +298,30 @@ void frame_written(sb_ctx* c, const sb_frame* f) {
   if (f == c->f_old || f == c->f_new || f == c->f_comp || f->id == c->memo.key.out) c->memo.clear();
 }
 
+// The host tier's tiles give their pinned buffers back for reuse (the copies that read them are ordered on the stream).
+void release_host_tile(sb_ctx* c, HostTile& h) {
+  c->tc.host_used -= h.count;
+  if (h.buf) c->tc.spare.emplace(h.cap, std::move(h.buf));
+}
+
+// A pinned buffer of at least h.count surfels for a host tile: a spare one when one is large enough, else a new one.
+int acquire_host_buffer(sb_ctx* c, HostTile& h) {
+  if (h.count == 0) return SB_OK;
+  auto sp = c->tc.spare.lower_bound(h.count);
+  if (sp != c->tc.spare.end()) {
+    h.cap = sp->first;
+    h.buf = std::move(sp->second);
+    c->tc.spare.erase(sp);
+    return SB_OK;
+  }
+  void* p = nullptr;
+  cudaError_t e = cudaMallocHost(&p, (size_t)h.count * 64);
+  if (e != cudaSuccess) return fail(c, SB_ERR_NOMEM, std::string("tile cache host tier: ") + cudaGetErrorString(e));
+  h.cap = h.count;
+  h.buf.reset(static_cast<float4*>(p));
+  return SB_OK;
+}
+
 int reset_state(sb_ctx* c) {
   // SurfelMap::reset (SurfelMap.cpp:473-482) + the SurfelMapping members set up in its constructor
   c->map_version += 1;
@@ -289,6 +332,10 @@ int reset_state(sb_ctx* c) {
   c->tiles.clear();
   c->n_slots = 0;
   c->tiles_pending = false;
+  for (auto& kv : c->tc.host) release_host_tile(c, kv.second);
+  c->tc.host.clear();
+  c->tc.pool_bound = 0;
+  c->tc.reclaims = c->tc.reclaim_moved = c->tc.evictions = c->tc.host_fills = c->tc.dropped_retired = 0;
   c->stats[12] = 0.0;
   c->loop.reset();  // posegraph_->clear(); trajectory_distances_ ... (SurfelMapping.cpp:158-163)
   for (int i = 0; i < 16; ++i) c->lastPose_old[i] = (i % 5 == 0) ? 1.0 : 0.0;
@@ -671,16 +718,21 @@ int fetch_counts(sb_ctx* c, uint32_t* dst, int n) {
   return SB_OK;
 }
 
-int refresh_tile_records(sb_ctx* c) {  // read back the records of the tiles extracted so far
-  if (!c->tiles_pending || c->n_slots == 0) return SB_OK;
-  std::vector<uint2> rec(c->n_slots);
+// read back the records of the tiles extracted so far (all of them into *out, if given, even when none is pending)
+int refresh_tile_records(sb_ctx* c, std::vector<uint2>* out = nullptr) {
+  if (out) out->clear();
+  if ((!c->tiles_pending && !out) || c->n_slots == 0) return SB_OK;
+  std::vector<uint2> local;
+  std::vector<uint2>& rec = out ? *out : local;
+  rec.resize(c->n_slots);
   SB_CUDA(c, cudaMemcpyAsync(rec.data(), c->d_tile_rec, (size_t)c->n_slots * sizeof(uint2), cudaMemcpyDeviceToHost,
                              c->stream));
   SB_CUDA(c, cudaStreamSynchronize(c->stream));
   auto base = [&](uint32_t s) { return s ? rec[s - 1].x : 0u; };
   {  // surfels that did not fit the 16 M-surfel HBM tile pool (the reference's host-side cache is unbounded); slots are
-     // never reused, so the sum over all slots counts every drop since the last reset
-    uint64_t dropped = 0;
+     // never reused, so the sum over all slots counts every drop since the last reset (a managed cache renumbers them
+     // and carries the drops of the retired slots in dropped_retired)
+    uint64_t dropped = c->tc.dropped_retired;
     for (uint32_t s = 0; s < c->n_slots; ++s) dropped += std::min(rec[s].y, kExtractCap) - (rec[s].x - base(s));
     if ((double)dropped != c->stats[12]) {
       c->stats[12] = (double)dropped;
@@ -696,6 +748,7 @@ int refresh_tile_records(sb_ctx* c) {  // read back the records of the tiles ext
     }
   }
   c->tiles_pending = false;
+  c->tc.pool_bound = c->n_slots ? rec[c->n_slots - 1].x : 0u;
   return SB_OK;
 }
 
@@ -724,19 +777,34 @@ int append_tiles(sb_ctx* c, int32_t i0, int32_t j0, int di, int dj) {  // Surfel
   int r;
   bool appended = false;
   for (int32_t k = -dim; k <= dim; ++k) {
-    auto it = c->tiles.find(std::make_pair(i0 + di * k, j0 + dj * k));
-    if (it == c->tiles.end()) continue;  // submapCache_[idx] of a tile never extracted: empty
-    if (!it->second.known && (r = refresh_tile_records(c))) return r;
-    const DevTile& t = it->second;
+    const std::pair<int32_t, int32_t> idx(i0 + di * k, j0 + dj * k);
+    auto it = c->tiles.find(idx);
+    const HostTile* h = nullptr;
+    if (it == c->tiles.end()) {
+      auto hi = c->tc.host.find(idx);
+      if (hi == c->tc.host.end()) continue;  // submapCache_[idx] of a tile never extracted: empty
+      h = &hi->second;  // a tile of the managed cache's host tier: it stays there until it is extracted again
+    } else if (!it->second.known && (r = refresh_tile_records(c))) {
+      return r;
+    }
+    const uint32_t count = h ? h->count : it->second.count;
     // the reference's map has no dead slots: a tile that does not fit behind them fits (or is cut) after compaction
-    if (t.count > kMaxSurfels - c->n_host && (r = compact_map(c))) return r;
+    if (count > kMaxSurfels - c->n_host && (r = compact_map(c))) return r;
     uint32_t room = kMaxSurfels - c->n_host;
-    uint32_t n = t.count < room ? t.count : room;
+    uint32_t n = count < room ? count : room;
     if (n == 0) continue;
-    // the four lanes of A and of the pool lie at fixed pitches (kMaxSurfels, kTilePoolCap) in one allocation each
-    for (size_t lane = 0; lane < 4; ++lane)
-      SB_CUDA(c, cudaMemcpyAsync(c->A.p0 + lane * kMaxSurfels + c->n_host, c->pool.p0 + lane * kTilePoolCap + t.base,
-                                 (size_t)n * 16, cudaMemcpyDeviceToDevice, c->stream));
+    // the four lanes of A and of the pool lie at fixed pitches (kMaxSurfels, kTilePoolCap) in one allocation each; those
+    // of a host tile at pitch count
+    for (size_t lane = 0; lane < 4; ++lane) {
+      if (h)
+        SB_CUDA(c, cudaMemcpyAsync(c->A.p0 + lane * kMaxSurfels + c->n_host, h->buf + lane * count, (size_t)n * 16,
+                                   cudaMemcpyHostToDevice, c->stream));
+      else
+        SB_CUDA(c, cudaMemcpyAsync(c->A.p0 + lane * kMaxSurfels + c->n_host,
+                                   c->pool.p0 + lane * kTilePoolCap + it->second.base, (size_t)n * 16,
+                                   cudaMemcpyDeviceToDevice, c->stream));
+    }
+    if (h) c->tc.host_fills += 1;
     SB_CUDA(c, cudaMemsetAsync(c->live + c->n_host, 1, n, c->stream));
     c->n_host += n;
     c->n_upper = c->n_host;
@@ -750,19 +818,166 @@ int append_tiles(sb_ctx* c, int32_t i0, int32_t j0, int di, int dj) {  // Surfel
   return SB_OK;
 }
 
+// ---- managed tile cache (DESIGN.md section 10) ----
+// Compacts the pool: the ranges of the cached tiles move to its front in pool order (through the idle scratch set T, in
+// rounds of at most kMaxSurfels, so that no range is read after it has been overwritten), their records become dense
+// again and their slots are renumbered 0 .. tiles - 1. rec: the records as on the device (every tile is known); updated.
+int reclaim_pool(sb_ctx* c, std::vector<uint2>& rec) {
+  sb_ctx::TileCache& tc = c->tc;
+  std::vector<DevTile*> order;
+  for (auto& kv : c->tiles) order.push_back(&kv.second);
+  std::sort(order.begin(), order.end(), [](const DevTile* a, const DevTile* b) { return a->slot < b->slot; });
+  const uint32_t end = c->n_slots ? rec[c->n_slots - 1].x : 0u;
+  uint64_t referenced = 0;
+  for (const DevTile* t : order) referenced += t->count;
+  if (referenced == end && order.size() == c->n_slots) {
+    tc.pool_bound = end;
+    return SB_OK;
+  }
+  // the drops of the slots that go away stay counted
+  for (uint32_t s = 0; s < c->n_slots; ++s)
+    tc.dropped_retired += std::min(rec[s].y, kExtractCap) - (rec[s].x - (s ? rec[s - 1].x : 0u));
+  // moves in pool order: (source, destination) runs of adjacent tiles; the tiles already in place stay
+  struct Run { uint32_t src, dst, n; };
+  std::vector<Run> runs;
+  std::vector<uint2> nrec(order.size());
+  uint32_t dst = 0;
+  for (size_t k = 0; k < order.size(); ++k) {
+    DevTile& t = *order[k];
+    if (t.count && t.base != dst) {
+      if (!runs.empty() && runs.back().src + runs.back().n == t.base && runs.back().dst + runs.back().n == dst)
+        runs.back().n += t.count;
+      else
+        runs.push_back(Run{t.base, dst, t.count});
+    }
+    t.slot = (uint32_t)k;
+    t.base = dst;
+    dst += t.count;
+    nrec[k] = make_uint2(dst, t.count);
+  }
+  // rounds: each gathers up to kMaxSurfels of the moved surfels into T and writes them back to their destination; a
+  // destination lies at or below its source, and the sources of later rounds lie above this round's destinations
+  std::vector<uint2> segs;
+  std::vector<uint32_t> seg_begin, round_dst, round_n;
+  uint32_t filled = 0;
+  for (const Run& run : runs)
+    for (uint32_t o = 0; o < run.n;) {
+      if (round_n.empty() || filled == kMaxSurfels) {
+        seg_begin.push_back((uint32_t)segs.size());
+        round_dst.push_back(run.dst + o);
+        round_n.push_back(0);
+        filled = 0;
+      }
+      const uint32_t n = std::min(run.n - o, kMaxSurfels - filled);
+      segs.push_back(make_uint2(run.src + o, filled));
+      filled += n;
+      round_n.back() += n;
+      o += n;
+    }
+  if (!segs.empty()) {
+    if (!tc.segs) SB_CUDA(c, dev_alloc(tc.segs, ((size_t)kMaxTileSlots + 64) * sizeof(uint2)));
+    SB_CUDA(c, cudaMemcpyAsync(tc.segs, segs.data(), segs.size() * sizeof(uint2), cudaMemcpyHostToDevice, c->stream));
+    Launch L = L_(c);
+    for (size_t q = 0; q < round_n.size(); ++q) {
+      const uint32_t s0 = seg_begin[q], s1 = q + 1 < round_n.size() ? seg_begin[q + 1] : (uint32_t)segs.size();
+      launch_pool_reclaim(L, c->pool, c->T, tc.segs + s0, s1 - s0, 0, 0, round_n[q]);
+      launch_pool_reclaim(L, c->T, c->pool, nullptr, 0, 0, round_dst[q], round_n[q]);
+    }
+  }
+  if (!nrec.empty())
+    SB_CUDA(c, cudaMemcpyAsync(c->d_tile_rec, nrec.data(), nrec.size() * sizeof(uint2), cudaMemcpyHostToDevice, c->stream));
+  SB_CUDA(c, cudaStreamSynchronize(c->stream));  // the copies read host vectors
+  rec = nrec;
+  c->n_slots = (uint32_t)order.size();
+  tc.pool_bound = dst;
+  tc.reclaims += 1;
+  for (uint32_t n : round_n) tc.reclaim_moved += n;
+  return SB_OK;
+}
+
+// Moves one pool tile to the host tier (its pool range is abandoned until the next reclaim).
+int evict_tile(sb_ctx* c, std::map<std::pair<int32_t, int32_t>, DevTile>::iterator it) {
+  sb_ctx::TileCache& tc = c->tc;
+  const DevTile& t = it->second;
+  HostTile h;
+  h.count = t.count;
+  int r;
+  if ((r = acquire_host_buffer(c, h))) return r;
+  if (t.count) {
+    for (size_t lane = 0; lane < 4; ++lane)
+      SB_CUDA(c, cudaMemcpyAsync(h.buf + lane * t.count, c->pool.p0 + lane * kTilePoolCap + t.base, (size_t)t.count * 16,
+                                 cudaMemcpyDeviceToHost, c->stream));
+  }
+  tc.host_used += t.count;
+  tc.evictions += 1;
+  tc.host[it->first] = std::move(h);
+  c->tiles.erase(it);
+  return SB_OK;
+}
+
+// The decision point before each extraction of a managed cache: the pool must take a whole tile (kExtractCap, its size
+// is known only once its record is read back) and a record slot. The host's bound settles it on most scans without a
+// read-back; otherwise: read the records back, reclaim, and move tiles to the host tier while the pool is still short.
+// Eviction order: the tile farthest from the window origin (Chebyshev distance in tile indices) first, the oldest
+// extraction (lowest slot, the pool order) among equals -- replicated state only, so striped ranks stay identical.
+int make_tile_room(sb_ctx* c) {
+  sb_ctx::TileCache& tc = c->tc;
+  if (tc.pool_bound + kExtractCap <= tc.pool_cap && c->n_slots < kMaxTileSlots) return SB_OK;
+  std::vector<uint2> rec;
+  int r;
+  if ((r = refresh_tile_records(c, &rec))) return r;
+  if ((r = reclaim_pool(c, rec))) return r;
+  const uint64_t need = tc.pool_bound + kExtractCap > tc.pool_cap ? tc.pool_bound + kExtractCap - tc.pool_cap : 0;
+  const uint32_t need_slots = c->n_slots >= kMaxTileSlots ? c->n_slots + 1 - kMaxTileSlots : 0;
+  if (need == 0 && need_slots == 0) return SB_OK;
+  using Key = std::pair<int32_t, int32_t>;
+  std::vector<std::pair<std::pair<int64_t, uint32_t>, Key>> cand;  // ((-distance, slot), tile)
+  for (const auto& kv : c->tiles) {
+    const int64_t d = std::max(std::llabs((long long)kv.first.first - c->origin_i),
+                               std::llabs((long long)kv.first.second - c->origin_j));
+    cand.push_back(std::make_pair(std::make_pair(-d, kv.second.slot), kv.first));
+  }
+  std::sort(cand.begin(), cand.end());
+  uint64_t freed = 0;
+  uint32_t freed_slots = 0;
+  for (const auto& e : cand) {
+    if (freed >= need && freed_slots >= need_slots) break;
+    auto it = c->tiles.find(e.second);
+    if (it->second.count == 0 && freed_slots >= need_slots) continue;  // an empty tile frees only a slot
+    if (tc.host_used + it->second.count > tc.host_cap) continue;       // does not fit the host tier
+    freed += it->second.count;
+    freed_slots += 1;
+    if ((r = evict_tile(c, it))) return r;
+  }
+  // (nothing moved: both tiers are full, and the extraction is cut as the default cache cuts it)
+  return freed_slots ? reclaim_pool(c, rec) : SB_OK;
+}
+
 // SurfelMap.cpp:708-742 + extract_surfels.vert: the tile is compacted into the HBM pool; nothing is read back here
 int extract_surfels(sb_ctx* c, bool partially) {
   Launch L = L_(c);
+  int r;
   while (!c->extraction.empty()) {
     std::pair<int32_t, int32_t> idx = c->extraction.back();
     c->extraction.pop_back();
+    if (c->tc.managed) {
+      // the new extraction replaces the tile's cached copy: drop it first, so that a reclaim can use its pool range
+      c->tiles.erase(idx);
+      auto hi = c->tc.host.find(idx);
+      if (hi != c->tc.host.end()) {
+        release_host_tile(c, hi->second);
+        c->tc.host.erase(hi);
+      }
+      if ((r = make_tile_room(c))) return r;
+      c->tc.pool_bound += kExtractCap;
+    }
     if (c->n_slots >= kMaxTileSlots) return fail(c, SB_ERR_CAPACITY, "tile cache: out of record slots");
     float2 ctr = submap_center(c, idx.first, idx.second);
     uint32_t slot = c->n_slots++;
     // extractions can follow each other with no per-pixel prologue in between to clear the group totals
     SB_CUDA(c, cudaMemsetAsync(c->group_counts, 0, kGroupCounts * 4, c->stream));
     launch_extract_to_pool(L, c->A, c->res->counts, c->live, c->n_host, c->poses, ctr, c->p.submap_extent, c->keep,
-                           c->block_counts, c->group_counts, c->pool, kTilePoolCap, c->d_tile_rec, slot, kExtractCap);
+                           c->block_counts, c->group_counts, c->pool, c->tc.pool_cap, c->d_tile_rec, slot, kExtractCap);
     DevTile t;
     t.slot = slot;
     t.known = false;
@@ -1612,6 +1827,48 @@ int sb_map_submap_origin(sb_ctx* c, int32_t* i, int32_t* j, uint32_t* pending) {
   return SB_OK;
 }
 
+int sb_set_tile_cache(sb_ctx* c, uint32_t pool_surfels, uint64_t host_surfels) {
+  if (!c) return SB_ERR_INVALID;
+  if (pool_surfels < kExtractCap || pool_surfels > kTilePoolCap)
+    return fail(c, SB_ERR_INVALID, "set_tile_cache: pool_surfels must lie in [500000, 16777216]");
+  if (c->n_slots != 0 || !c->tiles.empty() || !c->tc.host.empty())
+    return fail(c, SB_ERR_STATE, "set_tile_cache: the tile cache is not empty (call it after sb_create or sb_reset)");
+  c->tc.managed = true;
+  c->tc.pool_cap = pool_surfels;
+  c->tc.host_cap = host_surfels;
+  return SB_OK;
+}
+
+int sb_get_tile_cache_info(sb_ctx* c, sb_tile_cache_info* o) {
+  if (!c || !o) return SB_ERR_INVALID;
+  cudaSetDevice(c->device);
+  std::vector<uint2> rec(c->n_slots);
+  if (c->n_slots) {  // read the records without changing what the context knows
+    SB_CUDA(c, cudaMemcpyAsync(rec.data(), c->d_tile_rec, rec.size() * sizeof(uint2), cudaMemcpyDeviceToHost, c->stream));
+    SB_CUDA(c, cudaStreamSynchronize(c->stream));
+  }
+  memset(o, 0, sizeof(*o));
+  const sb_ctx::TileCache& tc = c->tc;
+  o->managed = tc.managed;
+  o->tiles_in_pool = (uint32_t)c->tiles.size();
+  o->tiles_on_host = (uint32_t)tc.host.size();
+  o->pool_capacity = tc.pool_cap;
+  o->pool_used = c->n_slots ? rec[c->n_slots - 1].x : 0u;
+  for (const auto& kv : c->tiles) {
+    const uint32_t s = kv.second.slot;
+    o->pool_referenced += rec[s].x - (s ? rec[s - 1].x : 0u);
+  }
+  o->host_capacity = tc.host_cap;
+  o->host_used = tc.host_used;
+  o->reclaims = tc.reclaims;
+  o->reclaim_moved = tc.reclaim_moved;
+  o->evictions = tc.evictions;
+  o->host_fills = tc.host_fills;
+  o->dropped = tc.dropped_retired;
+  for (uint32_t s = 0; s < c->n_slots; ++s) o->dropped += std::min(rec[s].y, kExtractCap) - (rec[s].x - (s ? rec[s - 1].x : 0u));
+  return SB_OK;
+}
+
 int sb_process_scan(sb_ctx* c, const float* pts4, const float* labels, const float* probs, uint32_t n, int on_device) {
   if (!c || (!pts4 && n)) return fail(c, SB_ERR_INVALID, "process_scan: null argument");
   cudaSetDevice(c->device);
@@ -1998,7 +2255,7 @@ static_assert(__BYTE_ORDER__ == __ORDER_LITTLE_ENDIAN__, "checkpoints are writte
 const char kStateMagic[8] = {'S', 'B', 'S', 'T', 'A', 'T', 'E', '\0'};
 constexpr uint32_t kStateFormat = 1;
 constexpr size_t kStageBytes = 16u << 20;  // one half of the pinned double buffer
-enum StateSection : uint32_t { S_HOST = 1, S_LOOP, S_POSES, S_RESULT, S_TILES, S_SURFELS, S_POOL, S_FRAMES };
+enum StateSection : uint32_t { S_HOST = 1, S_LOOP, S_POSES, S_RESULT, S_TILES, S_SURFELS, S_POOL, S_FRAMES, S_TCACHE };
 
 #define SB_PARAM_FIELDS(X)                                                                                              \
   X(data_width) X(data_height) X(data_fov_up) X(data_fov_down) X(min_depth) X(max_depth) X(model_width)                 \
@@ -2084,6 +2341,16 @@ struct StateImage {
   ResultBlock result;
   std::vector<uint2> tile_rec;
   lp::State loop;
+  // the managed tile cache (section S_TCACHE, written only by managed contexts)
+  struct HostTileImage {
+    int32_t i, j;
+    uint32_t count;
+    const uint8_t* data;  // count surfels as four lanes of pitch count: the pinned buffer (save) or the blob (load)
+  };
+  uint32_t tc_managed = 0, tc_pool_cap = kTilePoolCap;
+  uint64_t tc_host_cap = 0, tc_pool_bound = 0, tc_host_used = 0, tc_reclaims = 0, tc_moved = 0, tc_evictions = 0,
+           tc_fills = 0, tc_dropped = 0;
+  std::vector<HostTileImage> host_tiles;
 };
 
 void put_m4(Writer& w, const lp::M4& m) { w.bytes(m.m, sizeof(m.m)); }
@@ -2180,6 +2447,16 @@ void write_host_sections(Writer& w, const StateImage& s) {
   o = w.open(S_TILES);
   w.put((uint32_t)s.tile_rec.size());
   for (const uint2& r : s.tile_rec) { w.put(r.x); w.put(r.y); }
+  w.close(o);
+
+  if (!s.tc_managed) return;  // a default context's checkpoint has no such section
+  o = w.open(S_TCACHE);
+  w.put(s.tc_pool_cap); w.put((uint32_t)s.host_tiles.size());
+  for (uint64_t v : {s.tc_host_cap, s.tc_pool_bound, s.tc_host_used, s.tc_reclaims, s.tc_moved, s.tc_evictions, s.tc_fills,
+                     s.tc_dropped})
+    w.put(v);
+  for (const auto& t : s.host_tiles) { w.put(t.i); w.put(t.j); w.put(t.count); w.put(uint32_t(0)); }
+  for (const auto& t : s.host_tiles) w.bytes(t.data, (size_t)t.count * 64);
   w.close(o);
 }
 
@@ -2322,6 +2599,43 @@ const char* read_host(Reader& r, const sb_ctx* c, StateImage& s) {
     const uint32_t base = t.second.slot ? s.tile_rec[t.second.slot - 1].x : 0u;
     if (t.second.known && (t.second.base != base || t.second.count != s.tile_rec[t.second.slot].x - base))
       return "malformed tile table";
+  }
+
+  uint32_t next = 0;
+  if (r.n - r.off >= 4) memcpy(&next, r.p + r.off, 4);
+  if (next != S_TCACHE) return nullptr;
+  len = read_open(r, S_TCACHE);
+  start = r.off;
+  s.tc_managed = 1;
+  s.tc_pool_cap = r.get<uint32_t>();
+  s.host_tiles.resize(r.count(16));
+  for (uint64_t* v : {&s.tc_host_cap, &s.tc_pool_bound, &s.tc_host_used, &s.tc_reclaims, &s.tc_moved, &s.tc_evictions,
+                      &s.tc_fills, &s.tc_dropped})
+    *v = r.get<uint64_t>();
+  uint64_t host_total = 0;
+  for (auto& t : s.host_tiles) {
+    t.i = r.get<int32_t>(); t.j = r.get<int32_t>(); t.count = r.get<uint32_t>(); r.get<uint32_t>();
+    if (t.count > kExtractCap) return "malformed tile cache section (host tile over the extract cap)";
+    host_total += t.count;
+  }
+  if (!r.ok || host_total * 64 > r.n - r.off) return "malformed tile cache section";
+  for (auto& t : s.host_tiles) {
+    t.data = r.p + r.off;
+    r.off += (size_t)t.count * 64;
+  }
+  if (!read_close(r, start, len)) return "malformed tile cache section";
+  // every count is checked against the saved capacities before anything changes
+  if (s.tc_pool_cap < kExtractCap || s.tc_pool_cap > kTilePoolCap || s.pool_end > s.tc_pool_cap ||
+      s.tc_pool_bound < s.pool_end)
+    return "malformed tile cache section (pool beyond its capacity)";
+  if (host_total != s.tc_host_used || s.tc_host_used > s.tc_host_cap)
+    return "malformed tile cache section (host tier beyond its capacity)";
+  for (size_t k = 0; k < s.host_tiles.size(); ++k) {  // strictly ordered by index, none also in the pool
+    const auto key = std::make_pair(s.host_tiles[k].i, s.host_tiles[k].j);
+    if (k && !(std::make_pair(s.host_tiles[k - 1].i, s.host_tiles[k - 1].j) < key))
+      return "malformed tile cache section (host tiles out of order)";
+    for (const auto& t : s.tiles)
+      if (t.first == key) return "malformed tile cache section (a tile in both tiers)";
   }
   return nullptr;
 }
@@ -2473,6 +2787,15 @@ int capture(sb_ctx* c, StateImage& s) {
   if (c->n_slots)
     SB_CUDA(c, cudaMemcpy(s.tile_rec.data(), c->d_tile_rec, (size_t)c->n_slots * sizeof(uint2), cudaMemcpyDeviceToHost));
   s.pool_end = c->n_slots ? s.tile_rec[c->n_slots - 1].x : 0u;
+  const sb_ctx::TileCache& tc = c->tc;
+  s.tc_managed = tc.managed;
+  s.tc_pool_cap = tc.pool_cap;
+  s.tc_host_cap = tc.host_cap; s.tc_pool_bound = tc.pool_bound; s.tc_host_used = tc.host_used;
+  s.tc_reclaims = tc.reclaims; s.tc_moved = tc.reclaim_moved; s.tc_evictions = tc.evictions; s.tc_fills = tc.host_fills; s.tc_dropped = tc.dropped_retired;
+  s.host_tiles.clear();
+  for (const auto& kv : tc.host)  // (the stream is synchronised: the evictions' copies have landed)
+    s.host_tiles.push_back(StateImage::HostTileImage{kv.first.first, kv.first.second, kv.second.count,
+                                                     reinterpret_cast<const uint8_t*>(kv.second.buf.get())});
   // the used entries of the pose tables: those the map can refer to, and any set beyond them through sb_map_set_pose
   uint32_t np = pose_table_count(c);
   for (uint32_t t = kMaxPoses; t > np; --t) {
@@ -2492,8 +2815,37 @@ int capture(sb_ctx* c, StateImage& s) {
   return SB_OK;
 }
 
+// The host tier of a checkpoint replaces the context's (and with it the cache setting).
+int apply_tile_cache(sb_ctx* c, const StateImage& s) {
+  sb_ctx::TileCache& tc = c->tc;
+  for (auto& kv : tc.host) release_host_tile(c, kv.second);
+  tc.host.clear();
+  tc.host_used = 0;
+  tc.managed = s.tc_managed != 0;
+  tc.pool_cap = s.tc_managed ? s.tc_pool_cap : kTilePoolCap;
+  tc.host_cap = s.tc_host_cap;
+  tc.pool_bound = s.tc_managed ? s.tc_pool_bound : s.pool_end;
+  tc.reclaims = s.tc_reclaims; tc.reclaim_moved = s.tc_moved; tc.evictions = s.tc_evictions; tc.host_fills = s.tc_fills;
+  tc.dropped_retired = s.tc_dropped;
+  for (const auto& t : s.host_tiles) {
+    HostTile h;
+    h.count = t.count;
+    int r;
+    if ((r = acquire_host_buffer(c, h))) return r;
+    if (t.count) memcpy(h.buf.get(), t.data, (size_t)t.count * 64);
+    tc.host_used += t.count;
+    tc.host[std::make_pair(t.i, t.j)] = std::move(h);
+  }
+  return SB_OK;
+}
+
 // Commits a verified checkpoint (the bulk sections are already on the device).
 int apply(sb_ctx* c, const StateImage& s) {
+  if (int r = apply_tile_cache(c, s)) {
+    const std::string why = c->err;
+    reset_state(c);  // never leave a half-loaded context behind
+    return fail(c, r, why + "; the context was reset");
+  }
   c->p = s.p;
   derive(c);
   c->confidence_threshold = s.confidence_threshold;

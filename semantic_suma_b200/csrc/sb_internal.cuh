@@ -158,7 +158,7 @@ enum KernelId {
   K_FILL = 0, K_PROJECT_SCATTER, K_PREPROCESS_TILE, K_ICP_JACOBIAN, K_GN_INIT,
   K_ICP_FUSED, K_POSE_PRODUCTS, K_RENDER_SCATTER, K_RENDER_RESOLVE, K_INDEX_SCATTER, K_RADIUS, K_UPDATE_SURFELS,
   K_GEN_SURFELS, K_EXTRACT_FLAGS, K_COMPACT_SCATTER, K_AOS_TO_SOA, K_SOA_TO_AOS, K_ICP_POST, K_STATE_PACK,
-  K_STATE_UNPACK, K_STATE_DIGEST, K_COUNT
+  K_STATE_UNPACK, K_STATE_DIGEST, K_POOL_RECLAIM, K_COUNT
 };
 const char* kernel_name(int id);
 
@@ -305,6 +305,11 @@ void launch_extract_to_pool(const Launch& L, SurfelPlanes map, const uint32_t* n
                             const float* poses, float2 center, float extent, uint8_t* keep, uint32_t* block_counts,
                             uint32_t* group_counts, SurfelPlanes pool, uint32_t pool_cap, uint2* rec, uint32_t slot,
                             uint32_t tile_cap);
+// Managed tile cache: dst[dst_base + d] = src[segs[i].x + d - segs[i].y] for d in [0, total), i the last segment with
+// segs[i].y <= d (segs sorted by .y, segs[0].y == 0); nseg == 0: one segment that starts at src_base. src and dst must
+// not overlap (the pool is compacted through the scratch set T).
+void launch_pool_reclaim(const Launch& L, SurfelPlanes src, SurfelPlanes dst, const uint2* segs, uint32_t nseg,
+                         uint32_t src_base, uint32_t dst_base, uint32_t total);
 void launch_aos_to_soa(const Launch& L, const sb_surfel* aos, SurfelPlanes s, uint32_t offset, uint32_t n);
 void launch_soa_to_aos(const Launch& L, SurfelPlanes s, sb_surfel* aos, uint32_t n);
 

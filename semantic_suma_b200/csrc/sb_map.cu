@@ -27,7 +27,7 @@ const char* kernel_name(int id) {
                                        "icp_jacobian", "gn_init", "icp_fused", "pose_products", "render_scatter",
                                        "render_resolve", "index_scatter", "radius", "update_surfels", "gen_surfels",
                                        "extract_flags", "compact_scatter", "aos_to_soa", "soa_to_aos", "icp_post",
-                                       "state_pack", "state_unpack", "state_digest"};
+                                       "state_pack", "state_unpack", "state_digest", "pool_reclaim"};
   return (id >= 0 && id < K_COUNT) ? names[id] : "?";
 }
 
@@ -1373,6 +1373,41 @@ void launch_gen_compact(const Launch& L, const KParams& kp, FrameDev frame, cons
     k_gen_compact<<<(P + kThreads - 1) / kThreads, kThreads, 0, L.stream>>>(kp, frame, radius_map, integrated, poses,
                                                                            timestamp, submap_center, submap_extent, map,
                                                                            live, lazy_groups, lb, cap, counts);
+  }
+}
+
+// ---- managed tile cache: ordered segmented move of pool ranges (one thread per surfel, four 128-bit lanes). Segment
+// i covers [segs[i].y, segs[i + 1].y) of the destination range; the binary search runs over at most kMaxTileSlots entries.
+__global__ void __launch_bounds__(kThreads) k_pool_reclaim(SurfelPlanes src, SurfelPlanes dst, const uint2* __restrict__ segs,
+                                                          uint32_t nseg, uint32_t src_base, uint32_t dst_base,
+                                                          uint32_t total) {
+  for (uint32_t d = blockIdx.x * blockDim.x + threadIdx.x; d < total; d += gridDim.x * blockDim.x) {
+    uint32_t s = src_base + d;
+    if (nseg) {
+      uint32_t lo = 0, hi = nseg - 1;
+      while (lo < hi) {
+        const uint32_t mid = (lo + hi + 1) >> 1;
+        if (__ldg(&segs[mid].y) <= d) lo = mid; else hi = mid - 1;
+      }
+      const uint2 g = __ldg(&segs[lo]);
+      s = g.x + (d - g.y);
+    }
+    const uint32_t o = dst_base + d;
+    dst.p0[o] = src.p0[s];
+    dst.p1[o] = src.p1[s];
+    dst.p2[o] = src.p2[s];
+    dst.p3[o] = src.p3[s];
+  }
+}
+
+void launch_pool_reclaim(const Launch& L, SurfelPlanes src, SurfelPlanes dst, const uint2* segs, uint32_t nseg,
+                         uint32_t src_base, uint32_t dst_base, uint32_t total) {
+  if (total == 0) return;
+  uint32_t blocks = (total + kThreads - 1) / kThreads;
+  if (blocks > 132u * 16u) blocks = 132u * 16u;
+  {
+    ScopedKernel sk(L, K_POOL_RECLAIM);
+    k_pool_reclaim<<<blocks, kThreads, 0, L.stream>>>(src, dst, segs, nseg, src_base, dst_base, total);
   }
 }
 

@@ -14,6 +14,10 @@ to PATH and the trajectory so far to PATH.poses.npy, after every --save-every N 
 --resume PATH continues at the scan after the saved one. The pose file of a resumed run is byte-identical to the one of
 an uninterrupted run.
 
+Full sequences extract more submap tiles than the default HBM tile cache holds: --tile-cache-host N turns on the managed
+cache (sb_set_tile_cache) with up to N surfels in pinned host memory (inf: no bound, as the reference's cache; 0: the
+default cache). The run then prints the cache's counters.
+
 The engine is the CUDA library (an H100 is required); tests inject another engine through `make_engine` to check the
 file plumbing without a GPU.
 """
@@ -65,18 +69,36 @@ def read_checkpoint(engine, state_path):
     return poses
 
 
+def parse_host_surfels(text):
+    """--tile-cache-host: a surfel count, or inf for no bound"""
+    if text.strip().lower() in ("inf", "infinity"):
+        return float("inf")
+    n = int(text)
+    if n < 0:
+        raise ValueError("--tile-cache-host must be >= 0 or inf")
+    return n
+
+
+TILE_POOL_SURFELS = 16 * 1024 * 1024  # the HBM share of a managed tile cache: the whole pool
+
+
 def run_sequence(seq_dir, params, make_engine=None, semantic=False, max_scans=None, on_scan=None, save_state=None,
-                 save_every=None, resume=None):
-    """-> dict(poses=[4x4 float64 in the velodyne frame, from scan 0], seconds, scans processed by this call).
+                 save_every=None, resume=None, tile_cache_host=0):
+    """-> dict(poses=[4x4 float64 in the velodyne frame, from scan 0], seconds, scans processed by this call, and
+    tile_cache: the cache's counters when tile_cache_host is set).
     `make_engine(params)` must return an object with processScan(points4, labels, probs) and getCurrentPose() -- the
-    SurfelMapping surface -- and, for save_state / resume, save_state(), load_state(bytes) and timestamp().
-    resume: a checkpoint written by save_state; the run continues at the scan after it."""
+    SurfelMapping surface -- and, for save_state / resume, save_state(), load_state(bytes) and timestamp(); for
+    tile_cache_host, setTileCache(pool, host) and tile_cache_info().
+    resume: a checkpoint written by save_state; the run continues at the scan after it (with the cache it was saved with).
+    tile_cache_host: surfels the managed tile cache may keep in host memory (inf: no bound; 0: the default cache)."""
     files = list_scans(seq_dir)
     if max_scans is not None:
         files = files[:max_scans]
     if not files:
         raise FileNotFoundError("no scans under %s/velodyne" % seq_dir)
     engine = (make_engine or _cuda_engine)(params)
+    if tile_cache_host:
+        engine.setTileCache(TILE_POOL_SURFELS, tile_cache_host)
     poses = read_checkpoint(engine, resume) if resume else []
     first = len(poses)
     if first > len(files):
@@ -98,7 +120,10 @@ def run_sequence(seq_dir, params, make_engine=None, semantic=False, max_scans=No
             write_checkpoint(engine, save_state, poses)
     if save_state:
         write_checkpoint(engine, save_state, poses)
-    return {"poses": poses, "seconds": time.time() - t0, "scans": len(files) - first}
+    out = {"poses": poses, "seconds": time.time() - t0, "scans": len(files) - first}
+    if tile_cache_host:
+        out["tile_cache"] = engine.tile_cache_info()
+    return out
 
 
 def evaluate_against_ground_truth(seq_dir, poses_velo):
@@ -156,6 +181,8 @@ def main(argv=None, make_engine=None):
                     help="checkpoint file (and PATH.poses.npy): written at the end and every --save-every scans")
     ap.add_argument("--save-every", type=int, default=None, metavar="N")
     ap.add_argument("--resume", default=None, metavar="PATH", help="continue from a --save-state checkpoint")
+    ap.add_argument("--tile-cache-host", type=parse_host_surfels, default=0, metavar="N",
+                    help="managed submap tile cache with up to N surfels in host memory (inf: no bound; 0: default cache)")
     args = ap.parse_args(argv)
     if args.save_every is not None and (args.save_every <= 0 or not args.save_state):
         ap.error("--save-every needs --save-state and N > 0")
@@ -169,7 +196,8 @@ def main(argv=None, make_engine=None):
     from . import api
     params = api.default_params(data_width=args.width, model_width=args.width)
     res = run_sequence(args.seq, params, make_engine=make_engine, semantic=args.semantic, max_scans=args.max_scans,
-                       save_state=args.save_state, save_every=args.save_every, resume=args.resume)
+                       save_state=args.save_state, save_every=args.save_every, resume=args.resume,
+                       tile_cache_host=args.tile_cache_host)
     calib_file = os.path.join(args.seq, "calib.txt")
     Tr = kitti.read_calibration(calib_file).get("Tr") if os.path.exists(calib_file) else None
     if args.out:
@@ -177,6 +205,8 @@ def main(argv=None, make_engine=None):
     report = {"scans": res["scans"], "seconds": round(res["seconds"], 3),
               "scans_per_sec_incl_file_io": round(res["scans"] / res["seconds"], 2) if res["seconds"] > 0 else None,
               "odometry": evaluate_against_ground_truth(args.seq, res["poses"])}
+    if "tile_cache" in res:
+        report["tile_cache"] = res["tile_cache"]
     print(json.dumps(report))
     return 0
 
