@@ -193,6 +193,37 @@ int sb_get_tile_cache_info(sb_ctx* ctx, sb_tile_cache_info* out);
 /* ---- SurfelMapping::processScan, SurfelMapping.cpp:175-210 (loop closure off) ---------------------------------- */
 int sb_process_scan(sb_ctx* ctx, const float* pts4, const float* labels, const float* probs, uint32_t n,
                     int pts_on_device);
+/* ---- per-point deskewing (no counterpart in the reference; DESIGN.md section 11) ----------------------------------
+ * A spinning LiDAR measures its points over a whole sweep. With deskewing on, preprocessing first moves every point to
+ * the scan's reference time with the motion the next Gauss-Newton run starts from (M = lastIncrement_: identity at
+ * timestamp 0, after sb_reset and after a reset load; after sb_state_load what the checkpoint holds; the same with
+ * initialize_identity on or off; after a track-loss recovery the recovery's increment, as for the initial guess):
+ *   p' = Exp((s - s_ref) w) p + (s - s_ref) t,   w = log_SO3(R_M), t = t_M (fp64 once per scan, rounded to fp32)
+ * with s in [0, 1] the point's sweep time: mode 1 the caller's per-point time (clamped; non-finite -> s_ref), mode 2
+ * frac(dir (a0 - yaw) / 2pi) of the point's azimuth, dir = +1 for a clockwise spin (the defaults a0 = +pi, clockwise give
+ * the range image's column fraction). Everything after the projection sees p'. When s == s_ref or M rounds to the
+ * identity, the point's bits pass through: with zero motion deskewing on gives the bits of deskewing off. */
+typedef struct sb_deskew_params {
+  int32_t mode;        /* 0 off, 1 per-point times, 2 azimuth */
+  float ref_time;      /* s_ref in [0, 1]: the sweep time the scan's pose refers to */
+  float start_azimuth; /* a0, radians (mode 2) */
+  int32_t clockwise;   /* mode 2 */
+} sb_deskew_params;
+void sb_default_deskew(sb_deskew_params* p); /* off, 0.5, +pi, clockwise */
+/* SB_ERR_INVALID for a mode outside {0, 1, 2}, a ref_time outside [0, 1] or not finite, a non-finite start_azimuth.
+ * Valid at any time; kept across sb_reset; saved by sb_state_save when on (a checkpoint without it loads with it off). */
+int sb_set_deskew(sb_ctx* ctx, const sb_deskew_params* p);
+int sb_get_deskew(sb_ctx* ctx, sb_deskew_params* p);
+/* sb_process_scan with per-point times (float, one per point). times follow pts_on_device: device memory when it is set,
+ * host memory otherwise; sb_prefetch_scan does not stage them (this call uploads them itself). SB_ERR_INVALID, before
+ * anything changes, for mode 1 without times and for times while the mode is not 1. sb_process_scan is this call with
+ * times = NULL. */
+int sb_process_scan_timed(sb_ctx* ctx, const float* pts4, const float* labels, const float* probs, const float* times,
+                          uint32_t n, int pts_on_device);
+/* sb_preprocess with deskewing by an explicit motion (column-major, NULL = identity) and setting, for tests and tools */
+int sb_preprocess_deskew(sb_ctx* ctx, const float* pts4, const float* labels, const float* probs, const float* times,
+                         uint32_t n, uint32_t timestamp, const sb_deskew_params* d, const double motion[16],
+                         int pts_on_device, sb_frame* out);
 /* Optional input double buffering (no counterpart in the reference, which uploads inside processScan,
  * SurfelMapping.cpp:325-331): start the host-to-device copy of the NEXT scan on a separate copy stream; a following
  * sb_process_scan with the same host pointers / count (on_device = 0) uses the staged copy. At most two scans staged. */

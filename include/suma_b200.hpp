@@ -464,6 +464,13 @@ class SurfelMapping {
   /** managed submap tile cache: see SurfelMap::setTileCache */
   void setTileCache(uint32_t pool_surfels, uint64_t host_surfels) { map_->setTileCache(pool_surfels, host_surfels); }
   sb_tile_cache_info tileCacheInfo() const { return map_->tileCacheInfo(); }
+  /** per-point deskewing of every scan (sb_set_deskew; no counterpart in the reference) */
+  void setDeskew(const sb_deskew_params& d) { check(sb_set_deskew(ctx_->get(), &d), ctx_->get(), "SurfelMapping::setDeskew"); }
+  sb_deskew_params getDeskew() const {
+    sb_deskew_params d;
+    check(sb_get_deskew(ctx_->get(), &d), ctx_->get(), "SurfelMapping::getDeskew");
+    return d;
+  }
   void reset() {
     check(sb_reset(ctx_->get()), ctx_->get(), "SurfelMapping::reset");
     trajectory_.clear();
@@ -472,6 +479,15 @@ class SurfelMapping {
   void processScan(const Laserscan& scan) {
     check(sb_process_scan(ctx_->get(), scan.points.data(), scan.labels_float.empty() ? nullptr : scan.labels_float.data(),
                           scan.labels_prob.empty() ? nullptr : scan.labels_prob.data(), scan.size(), 0),
+          ctx_->get(), "SurfelMapping::processScan");
+    trajectory_.push_back(getCurrentPose());
+  }
+  /** processScan with one sweep time per point (deskewing mode 1; host memory, scan.size() values) */
+  void processScan(const Laserscan& scan, const std::vector<float>& times) {
+    if (times.size() != scan.size()) throw std::invalid_argument("SurfelMapping::processScan: one time per point");
+    check(sb_process_scan_timed(ctx_->get(), scan.points.data(),
+                                scan.labels_float.empty() ? nullptr : scan.labels_float.data(),
+                                scan.labels_prob.empty() ? nullptr : scan.labels_prob.data(), times.data(), scan.size(), 0),
           ctx_->get(), "SurfelMapping::processScan");
     trajectory_.push_back(getCurrentPose());
   }

@@ -48,6 +48,22 @@ class TileCacheInfo(C.Structure):  # sb_tile_cache_info
 HOST_UNBOUNDED = 2**64 - 1  # sb_set_tile_cache: no bound on the host tier
 
 
+class DeskewParams(C.Structure):  # sb_deskew_params
+    _fields_ = [("mode", C.c_int32), ("ref_time", C.c_float), ("start_azimuth", C.c_float), ("clockwise", C.c_int32)]
+
+
+DESKEW_MODES = {"off": 0, "times": 1, "azimuth": 2}
+
+
+def deskew_params(mode="off", ref_time=0.5, start_azimuth=np.pi, clockwise=True):
+    """sb_deskew_params; mode: 0 / "off", 1 / "times" (per-point times), 2 / "azimuth" """
+    d = DeskewParams()
+    lib().sb_default_deskew(C.byref(d))
+    d.mode = DESKEW_MODES.get(mode, mode) if isinstance(mode, str) else int(mode)
+    d.ref_time, d.start_azimuth, d.clockwise = ref_time, start_azimuth, 1 if clockwise else 0
+    return d
+
+
 class Params(C.Structure):
     _fields_ = [
         ("data_width", C.c_int32), ("data_height", C.c_int32),
@@ -157,6 +173,9 @@ def lib(build_if_missing=True):
         "sb_state_size": [vp, C.POINTER(C.c_uint64)], "sb_state_save": [vp, vp, C.c_uint64, C.POINTER(C.c_uint64)],
         "sb_state_load": [vp, vp, C.c_uint64],
         "sb_set_tile_cache": [vp, u32, C.c_uint64], "sb_get_tile_cache_info": [vp, C.POINTER(TileCacheInfo)],
+        "sb_set_deskew": [vp, C.POINTER(DeskewParams)], "sb_get_deskew": [vp, C.POINTER(DeskewParams)],
+        "sb_process_scan_timed": [vp, vp, vp, vp, vp, u32, C.c_int],
+        "sb_preprocess_deskew": [vp, vp, vp, vp, vp, u32, u32, C.POINTER(DeskewParams), pd, C.c_int, vp],
     }
     for name, args in sig.items():
         fn = getattr(L, name)
@@ -170,6 +189,7 @@ def lib(build_if_missing=True):
     L.sb_se3_exp.argtypes = [pd, pd]; L.sb_se3_exp.restype = None
     L.sb_se3_log.argtypes = [pd, pd]; L.sb_se3_log.restype = None
     L.sb_icp_unpack.argtypes = [C.POINTER(C.c_int64), pd]; L.sb_icp_unpack.restype = None
+    L.sb_default_deskew.argtypes = [C.POINTER(DeskewParams)]; L.sb_default_deskew.restype = None
     _lib = L
     return L
 
@@ -188,6 +208,7 @@ EXPORTED_SYMBOLS = [
     "sb_set_current_pose", "sb_integrate_loop_closures",
     "sb_profile_kernels", "sb_profile_name", "sb_profile_collect", "sb_state_size", "sb_state_save", "sb_state_load",
     "sb_set_tile_cache", "sb_get_tile_cache_info",
+    "sb_default_deskew", "sb_set_deskew", "sb_get_deskew", "sb_process_scan_timed", "sb_preprocess_deskew",
 ]
 
 
@@ -295,6 +316,18 @@ class Context:
         self.check(lib().sb_set_params(self.h, C.byref(params)), "set_params")
         self.params = params
 
+    def set_deskew(self, mode="off", ref_time=0.5, start_azimuth=np.pi, clockwise=True):
+        """per-point deskewing of the scans (sb_set_deskew): mode "off" / "times" / "azimuth" (or 0 / 1 / 2)"""
+        d = deskew_params(mode, ref_time, start_azimuth, clockwise)
+        self.check(lib().sb_set_deskew(self.h, C.byref(d)), "set_deskew")
+
+    def get_deskew(self):
+        """the deskewing setting in effect as a dict (sb_get_deskew)"""
+        d = DeskewParams()
+        self.check(lib().sb_get_deskew(self.h, C.byref(d)), "get_deskew")
+        return {"mode": int(d.mode), "ref_time": float(d.ref_time), "start_azimuth": float(d.start_azimuth),
+                "clockwise": bool(d.clockwise)}
+
 
 class Frame:
     """core/Frame.h:21-79 -- vertex / normal / semantic maps living on the device."""
@@ -347,12 +380,22 @@ class Preprocessing:
     def __init__(self, ctx):
         self.ctx = ctx
 
-    def process(self, points, frame, labels=None, probs=None, timestamp=100):
+    def process(self, points, frame, labels=None, probs=None, timestamp=100, times=None, deskew=None, motion=None):
+        """deskew: None (the points as they are), or a DeskewParams / dict of deskew_params() arguments, with
+        motion = the sweep's 4x4 motion (None = identity) and times = the per-point sweep times of mode 1"""
         pts = np.ascontiguousarray(points, np.float32)
         lab = None if labels is None else np.ascontiguousarray(labels, np.float32)
         prb = None if probs is None else np.ascontiguousarray(probs, np.float32)
-        self.ctx.check(lib().sb_preprocess(self.ctx.h, _vp(pts), _vp(lab), _vp(prb), pts.shape[0], timestamp, 0, frame.h),
-                       "preprocess")
+        if deskew is None and times is None and motion is None:
+            self.ctx.check(lib().sb_preprocess(self.ctx.h, _vp(pts), _vp(lab), _vp(prb), pts.shape[0], timestamp, 0,
+                                               frame.h), "preprocess")
+            return
+        d = deskew if isinstance(deskew, DeskewParams) else deskew_params(**(deskew or {}))
+        tms = None if times is None else np.ascontiguousarray(times, np.float32)
+        m = None if motion is None else colmajor(motion, np.float64)
+        self.ctx.check(lib().sb_preprocess_deskew(self.ctx.h, _vp(pts), _vp(lab), _vp(prb), _vp(tms), pts.shape[0],
+                                                  timestamp, C.byref(d), None if m is None else _dp(m), 0, frame.h),
+                       "preprocess_deskew")
 
 
 class Frame2Model:
@@ -622,17 +665,28 @@ class SurfelMapping:
         """SurfelMapping::setCurrentPose (core/SurfelMapping.h:66)"""
         self.ctx.check(lib().sb_set_current_pose(self.ctx.h, _dp(colmajor(pose, np.float64))), "set_current_pose")
 
-    def processScan(self, points, labels=None, probs=None, on_device=False):
+    def processScan(self, points, labels=None, probs=None, on_device=False, times=None):
+        """times: per-point sweep times for deskewing mode 1 (setDeskew); with on_device a device pointer (int)"""
         if on_device:  # raw device pointers (int) + count: (ptr_pts, ptr_labels, ptr_probs, n)
             pp, pl, pq, n = points
-            rc = lib().sb_process_scan(self.ctx.h, C.c_void_p(pp), C.c_void_p(pl) if pl else None,
-                                       C.c_void_p(pq) if pq else None, n, 1)
+            tp = C.c_void_p(times) if times else None
+            rc = lib().sb_process_scan_timed(self.ctx.h, C.c_void_p(pp), C.c_void_p(pl) if pl else None,
+                                             C.c_void_p(pq) if pq else None, tp, n, 1)
         else:
             pts = np.ascontiguousarray(points, np.float32)
             lab = None if labels is None else np.ascontiguousarray(labels, np.float32)
             prb = None if probs is None else np.ascontiguousarray(probs, np.float32)
-            rc = lib().sb_process_scan(self.ctx.h, _vp(pts), _vp(lab), _vp(prb), pts.shape[0], 0)
+            tms = None if times is None else np.ascontiguousarray(times, np.float32)
+            rc = lib().sb_process_scan_timed(self.ctx.h, _vp(pts), _vp(lab), _vp(prb), _vp(tms), pts.shape[0], 0)
         self.ctx.check(rc, "process_scan")
+
+    def setDeskew(self, mode="off", ref_time=0.5, start_azimuth=np.pi, clockwise=True):
+        """Per-point deskewing of every scan with the motion of the previous increment (sb_set_deskew): mode "off",
+        "times" (processScan(..., times=...)) or "azimuth" (sweep time from each point's azimuth)"""
+        self.ctx.set_deskew(mode, ref_time, start_azimuth, clockwise)
+
+    def getDeskew(self):
+        return self.ctx.get_deskew()
 
     def process_scan_raw(self, ptr_pts, ptr_labels, ptr_probs, n, on_device):
         rc = lib().sb_process_scan(self.ctx.h, C.c_void_p(ptr_pts), C.c_void_p(ptr_labels) if ptr_labels else None,

@@ -15,6 +15,7 @@
 
 #include "sb_gn.cuh"
 #include "sb_internal.cuh"
+#include "../../include/suma_b200_deskew.h"
 #include "../../include/suma_b200_loop.hpp"
 
 using namespace sb;
@@ -71,6 +72,12 @@ struct sb_ctx {
   };
   PrefetchSlot prefetch[3];
   cudaStream_t copy_stream = nullptr;
+  // per-point deskewing (sb_set_deskew; DESIGN.md section 11): off by default, kept across sb_reset. The moved points and
+  // the uploaded per-point times live in buffers of desk_cap points, allocated on the first deskewed scan.
+  sb_deskew_params deskew{0, 0.5f, 3.14159265358979323846f, 1};
+  DevPtr<float4> d_desk;
+  DevPtr<float> d_times;
+  size_t desk_cap = 0;
 
   // ---- ICP
   DevPtr<GnState> gn;
@@ -1167,6 +1174,57 @@ int upload_scan(sb_ctx* c, const float* pts4, const float* labels, const float* 
   return SB_OK;
 }
 
+// ---- per-point deskewing (DESIGN.md section 11) ----
+const char* check_deskew(const sb_deskew_params* d) {
+  if (!d) return "null argument";
+  if (d->mode < 0 || d->mode > 2) return "mode must be 0 (off), 1 (per-point times) or 2 (azimuth)";
+  if (!(d->ref_time >= 0.0f && d->ref_time <= 1.0f)) return "ref_time must be a finite value in [0, 1]";
+  if (!std::isfinite(d->start_azimuth)) return "start_azimuth must be finite";
+  return nullptr;
+}
+// per-point times go with mode 1 and only with it (checked before anything changes)
+const char* check_deskew_times(const sb_deskew_params& d, const float* times) {
+  if (d.mode == 1 && !times) return "deskew mode 1 needs per-point times";
+  if (d.mode != 1 && times) return "per-point times are only read in deskew mode 1";
+  return nullptr;
+}
+
+// K1a's deskewing of a scan of n points moving by M over the sweep. *active stays false when nothing moves (mode 0, no
+// points, or a motion that rounds to zero): the scan then takes the plain projection, whose bits deskewing would give too.
+int setup_deskew(sb_ctx* c, const sb_deskew_params& d, const double* M, const float* times, uint32_t n, int on_device,
+                 DeskewArgs* a, bool* active) {
+  *active = false;
+  if (d.mode == 0 || n == 0) return SB_OK;
+  float w[3], t[3];
+  if (sb_deskew_motion(M, w, t)) return SB_OK;
+  if (c->desk_cap < n) {  // grows like the point buffers; the old buffers may still be read by the scan in flight
+    const size_t cap = std::max(c->pts_cap, (size_t)n + n / 4 + 1024);
+    SB_CUDA(c, cudaStreamSynchronize(c->stream));
+    DevPtr<float4> np;
+    DevPtr<float> nt;
+    if (dev_alloc(np, cap * 16) != cudaSuccess || dev_alloc(nt, cap * 4) != cudaSuccess) {
+      cudaGetLastError();
+      return fail(c, SB_ERR_CAPACITY, "out of device memory for the deskewing buffers");
+    }
+    c->d_desk = std::move(np);
+    c->d_times = std::move(nt);
+    c->desk_cap = cap;
+  }
+  const float* dt = nullptr;
+  if (d.mode == 1) {  // the times follow pts_on_device; sb_prefetch_scan does not stage them
+    if (on_device) {
+      dt = times;
+    } else {
+      SB_CUDA(c, cudaMemcpyAsync(c->d_times, times, (size_t)n * 4, cudaMemcpyHostToDevice, c->stream));
+      dt = c->d_times;
+    }
+  }
+  *a = DeskewArgs{dt, d.mode, d.ref_time, d.start_azimuth, d.clockwise != 0 ? 1 : 0, {w[0], w[1], w[2]},
+                  {t[0], t[1], t[2]}, c->d_desk};
+  *active = true;
+  return SB_OK;
+}
+
 // SurfelMap::render_composed, SurfelMap.cpp:1116-1165
 int render_composed_internal(sb_ctx* c, const float* pose_old, const float* pose_new, float conf_thr) {
   frame_written(c, c->f_comp);
@@ -1621,6 +1679,50 @@ int sb_preprocess(sb_ctx* c, const float* pts4, const float* labels, const float
   return SB_OK;
 }
 
+int sb_preprocess_deskew(sb_ctx* c, const float* pts4, const float* labels, const float* probs, const float* times,
+                         uint32_t n, uint32_t timestamp, const sb_deskew_params* d, const double motion[16],
+                         int on_device, sb_frame* out) {
+  if (!c || !out || (!pts4 && n)) return fail(c, SB_ERR_INVALID, "preprocess_deskew: null argument");
+  if (const char* why = check_deskew(d)) return fail(c, SB_ERR_INVALID, std::string("preprocess_deskew: ") + why);
+  if (const char* why = check_deskew_times(*d, times))
+    return fail(c, SB_ERR_INVALID, std::string("preprocess_deskew: ") + why);
+  if (out->d.W != c->kp.W || out->d.H != c->kp.H) return fail(c, SB_ERR_INVALID, "preprocess_deskew: frame size mismatch");
+  cudaSetDevice(c->device);
+  const float4* dp; const float* dl; const float* dq;
+  int r = upload_scan(c, pts4, labels, probs, n, on_device, &dp, &dl, &dq);
+  if (r) return r;
+  double I[16];
+  ident_d(I);
+  DeskewArgs da;
+  bool active = false;
+  if ((r = setup_deskew(c, *d, motion ? motion : I, times, n, on_device, &da, &active))) return r;
+  frame_written(c, out);
+  launch_preprocess(L_(c), c->kp, dp, dl, dq, n, timestamp, c->prep, out->d, nullptr, nullptr, nullptr, nullptr,
+                    active ? &da : nullptr);
+  SB_CUDA(c, cudaGetLastError());
+  return SB_OK;
+}
+
+void sb_default_deskew(sb_deskew_params* p) {
+  if (!p) return;
+  p->mode = 0;
+  p->ref_time = 0.5f;
+  p->start_azimuth = 3.14159265358979323846f;
+  p->clockwise = 1;
+}
+int sb_set_deskew(sb_ctx* c, const sb_deskew_params* p) {
+  if (!c) return SB_ERR_INVALID;
+  if (const char* why = check_deskew(p)) return fail(c, SB_ERR_INVALID, std::string("set_deskew: ") + why);
+  c->deskew = *p;
+  c->deskew.clockwise = p->clockwise != 0 ? 1 : 0;
+  return SB_OK;
+}
+int sb_get_deskew(sb_ctx* c, sb_deskew_params* p) {
+  if (!c || !p) return fail(c, SB_ERR_INVALID, "get_deskew: null argument");
+  *p = c->deskew;
+  return SB_OK;
+}
+
 int sb_map_render(sb_ctx* c, const float pose_old[16], const float pose_new[16], float conf_thr, sb_frame* out) {
   if (!c || !pose_old || !pose_new || !out) return fail(c, SB_ERR_INVALID, "map_render: null argument");
   if (out->d.W != c->kp.Wm || out->d.H != c->kp.Hm) return fail(c, SB_ERR_INVALID, "map_render: frame size mismatch");
@@ -1870,7 +1972,13 @@ int sb_get_tile_cache_info(sb_ctx* c, sb_tile_cache_info* o) {
 }
 
 int sb_process_scan(sb_ctx* c, const float* pts4, const float* labels, const float* probs, uint32_t n, int on_device) {
+  return sb_process_scan_timed(c, pts4, labels, probs, nullptr, n, on_device);
+}
+
+int sb_process_scan_timed(sb_ctx* c, const float* pts4, const float* labels, const float* probs, const float* times,
+                          uint32_t n, int on_device) {
   if (!c || (!pts4 && n)) return fail(c, SB_ERR_INVALID, "process_scan: null argument");
+  if (const char* why = check_deskew_times(c->deskew, times)) return fail(c, SB_ERR_INVALID, std::string("process_scan: ") + why);
   cudaSetDevice(c->device);
   const sb_params& p = c->p;
   Launch L = L_(c);
@@ -1879,6 +1987,10 @@ int sb_process_scan(sb_ctx* c, const float* pts4, const float* labels, const flo
   const float4* dp; const float* dl; const float* dq;
   int r = upload_scan(c, pts4, labels, probs, n, on_device, &dp, &dl, &dq);
   if (r) return r;
+  // deskewing with the motion the next Gauss-Newton run starts from: lastIncrement_ as the previous scan left it
+  DeskewArgs da;
+  bool deskew = false;
+  if ((r = setup_deskew(c, c->deskew, c->lastIncrement, times, n, on_device, &da, &deskew))) return r;
   // initialize(), SurfelMapping.cpp:323-331
   std::swap(c->cur, c->last);
   std::swap(c->cur_model, c->last_model);
@@ -1888,7 +2000,7 @@ int sb_process_scan(sb_ctx* c, const float* pts4, const float* labels, const flo
   // preprocess(), :342-358
   frame_written(c, c->cur);
   launch_preprocess(L, c->kp, dp, dl, dq, n, c->timestamp, c->prep, c->cur->d, c->radius_map, c->key_index, c->integrated,
-                    c->group_counts);
+                    c->group_counts, deskew ? &da : nullptr);
   c->prepped_for_update = true;
   float ct = conf_threshold(c);
   float Pold[16], Pnew[16];
@@ -2255,7 +2367,8 @@ static_assert(__BYTE_ORDER__ == __ORDER_LITTLE_ENDIAN__, "checkpoints are writte
 const char kStateMagic[8] = {'S', 'B', 'S', 'T', 'A', 'T', 'E', '\0'};
 constexpr uint32_t kStateFormat = 1;
 constexpr size_t kStageBytes = 16u << 20;  // one half of the pinned double buffer
-enum StateSection : uint32_t { S_HOST = 1, S_LOOP, S_POSES, S_RESULT, S_TILES, S_SURFELS, S_POOL, S_FRAMES, S_TCACHE };
+enum StateSection : uint32_t { S_HOST = 1, S_LOOP, S_POSES, S_RESULT, S_TILES, S_SURFELS, S_POOL, S_FRAMES, S_TCACHE,
+                               S_DESKEW };
 
 #define SB_PARAM_FIELDS(X)                                                                                              \
   X(data_width) X(data_height) X(data_fov_up) X(data_fov_down) X(min_depth) X(max_depth) X(model_width)                 \
@@ -2351,6 +2464,8 @@ struct StateImage {
   uint64_t tc_host_cap = 0, tc_pool_bound = 0, tc_host_used = 0, tc_reclaims = 0, tc_moved = 0, tc_evictions = 0,
            tc_fills = 0, tc_dropped = 0;
   std::vector<HostTileImage> host_tiles;
+  // the deskewing setting (section S_DESKEW, written only when deskewing is on)
+  sb_deskew_params deskew{0, 0.5f, 3.14159265358979323846f, 1};
 };
 
 void put_m4(Writer& w, const lp::M4& m) { w.bytes(m.m, sizeof(m.m)); }
@@ -2394,6 +2509,13 @@ void write_header(Writer& w, const StateImage& s, uint64_t total) {
   SB_LOOP_PARAM_FIELDS(X)
 #undef X
   w.align8();
+}
+
+void write_deskew_section(Writer& w, const StateImage& s) {
+  if (s.deskew.mode == 0) return;  // a context without deskewing writes no such section
+  size_t o = w.open(S_DESKEW);
+  w.put(s.deskew.mode); w.put(s.deskew.ref_time); w.put(s.deskew.start_azimuth); w.put(s.deskew.clockwise);
+  w.close(o);
 }
 
 void write_host_sections(Writer& w, const StateImage& s) {
@@ -2449,7 +2571,7 @@ void write_host_sections(Writer& w, const StateImage& s) {
   for (const uint2& r : s.tile_rec) { w.put(r.x); w.put(r.y); }
   w.close(o);
 
-  if (!s.tc_managed) return;  // a default context's checkpoint has no such section
+  if (!s.tc_managed) return write_deskew_section(w, s);  // a default context's checkpoint has no such section
   o = w.open(S_TCACHE);
   w.put(s.tc_pool_cap); w.put((uint32_t)s.host_tiles.size());
   for (uint64_t v : {s.tc_host_cap, s.tc_pool_bound, s.tc_host_used, s.tc_reclaims, s.tc_moved, s.tc_evictions, s.tc_fills,
@@ -2458,6 +2580,7 @@ void write_host_sections(Writer& w, const StateImage& s) {
   for (const auto& t : s.host_tiles) { w.put(t.i); w.put(t.j); w.put(t.count); w.put(uint32_t(0)); }
   for (const auto& t : s.host_tiles) w.bytes(t.data, (size_t)t.count * 64);
   w.close(o);
+  write_deskew_section(w, s);
 }
 
 // Opens section `id` and returns its payload length (0 and r.ok = false when the next section is another one).
@@ -2472,6 +2595,14 @@ bool read_close(Reader& r, size_t start, uint64_t len) {
   r.align8();
   return r.ok && r.off - start == len;
 }
+
+// id of the section that starts at the reader's offset (0 at the end of the buffer)
+uint32_t peek_section(const Reader& r) {
+  uint32_t next = 0;
+  if (r.ok && r.n - r.off >= 4) memcpy(&next, r.p + r.off, 4);
+  return next;
+}
+const char* read_tile_cache(Reader& r, StateImage& s);
 
 // Parses the header and the host sections; nullptr when they are well formed, otherwise the reason.
 const char* read_host(Reader& r, const sb_ctx* c, StateImage& s) {
@@ -2601,11 +2732,25 @@ const char* read_host(Reader& r, const sb_ctx* c, StateImage& s) {
       return "malformed tile table";
   }
 
-  uint32_t next = 0;
-  if (r.n - r.off >= 4) memcpy(&next, r.p + r.off, 4);
-  if (next != S_TCACHE) return nullptr;
-  len = read_open(r, S_TCACHE);
+  if (peek_section(r) == S_TCACHE)
+    if (const char* why = read_tile_cache(r, s)) return why;
+  if (peek_section(r) != S_DESKEW) return nullptr;  // a checkpoint without the section loads with deskewing off
+  len = read_open(r, S_DESKEW);
   start = r.off;
+  s.deskew.mode = r.get<int32_t>();
+  s.deskew.ref_time = r.get<float>();
+  s.deskew.start_azimuth = r.get<float>();
+  s.deskew.clockwise = r.get<int32_t>();
+  if (!read_close(r, start, len)) return "malformed deskew section";
+  if (check_deskew(&s.deskew) || s.deskew.mode == 0 || (s.deskew.clockwise != 0 && s.deskew.clockwise != 1))
+    return "malformed deskew section (setting out of range)";
+  return nullptr;
+}
+
+// The managed tile cache's section: the setting, the counters and the host tiles, range-checked.
+const char* read_tile_cache(Reader& r, StateImage& s) {
+  uint64_t len = read_open(r, S_TCACHE);
+  const size_t start = r.off;
   s.tc_managed = 1;
   s.tc_pool_cap = r.get<uint32_t>();
   s.host_tiles.resize(r.count(16));
@@ -2812,6 +2957,7 @@ int capture(sb_ctx* c, StateImage& s) {
   s.result.counts[0] = s.n_live;  // the map is restored dense: its physical end is the live count, no dead slots
   s.result.counts[5] = 0;
   s.loop = c->loop;
+  s.deskew = c->deskew;
   return SB_OK;
 }
 
@@ -2859,6 +3005,7 @@ int apply(sb_ctx* c, const StateImage& s) {
   c->cur_has_semantics = s.cur_has_semantics != 0; c->last_has_semantics = s.last_has_semantics != 0;
   c->close_loops = s.close_loops != 0;
   c->loop = s.loop;
+  c->deskew = s.deskew;
   c->n_host = s.n_live; c->n_holes = 0; c->lazy_update = false; c->n_upper = s.n_live;
   c->prepped_for_update = false;
   c->map_timestamp = s.map_timestamp; c->pose_ref_end = s.pose_ref_end;

@@ -208,10 +208,22 @@ struct PrepKeys {
 };
 size_t preprocess_key_elems(int W, int H);
 bool make_key_tensor_map(CUtensorMap* out, const unsigned long long* keys, int W, int H);
-// K1-K3 (+ optionally K6b radius map and the re-arming of the index-map keys / integrated flags for the map update)
+// per-point deskewing fused into K1a (DESIGN.md section 11): sweep-time source, s_ref, the sweep's motion as fp32
+// axis-angle w and translation t, and where the moved points go (n float4, read by the tile pass instead of the input)
+struct DeskewArgs {
+  const float* times;  // mode 1: device pointer, one time per point
+  int mode;            // 1 per-point times, 2 azimuth
+  float ref_time, start_azimuth;
+  int clockwise;
+  float w[3], t[3];
+  float4* out;
+};
+// K1-K3 (+ optionally K6b radius map and the re-arming of the index-map keys / integrated flags for the map update);
+// deskew == nullptr: the points are projected as they are
 void launch_preprocess(const Launch& L, const KParams& kp, const float4* pts, const float* labels, const float* probs,
                        uint32_t n, uint32_t timestamp, PrepKeys& keys, FrameDev out, float4* radius_map,
-                       unsigned long long* index_keys, uint8_t* integrated, uint32_t* group_counts);
+                       unsigned long long* index_keys, uint8_t* integrated, uint32_t* group_counts,
+                       const DeskewArgs* deskew = nullptr);
 
 // sb_icp.cu
 void launch_icp_jacobian(const Launch& L, const KParams& kp, const IcpArgs& a, const Mat4& pose, int iteration,

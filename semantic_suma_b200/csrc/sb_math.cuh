@@ -286,6 +286,37 @@ SB_HD void project01(V3 p, float fov_up, float fov, float min_depth, float max_d
   z = (depth - min_depth) / (max_depth - min_depth);
 }
 
+// ---- per-point deskewing (DESIGN.md section 11; restated by the oracle in orc_deskew.c) ----
+// Sweep time s in [0, 1] of a point. mode 1: the caller's time, clamped, a non-finite one counts as s_ref. mode 2: the
+// azimuth fraction frac(dir (a0 - yaw) / 2pi) of the raw point's yaw, dir = +1 for a clockwise spin.
+SB_HD float deskew_sweep_time(int mode, float t, float yaw, float ref, float a0, int clockwise) {
+  if (mode == 1) {
+    if (!(fabsf(t) <= 3.402823466e38f)) return ref;
+    return t < 0.0f ? 0.0f : (t > 1.0f ? 1.0f : t);
+  }
+  const float u = clockwise ? a0 - yaw : yaw - a0;
+  const float q = u / 6.28318530717958647692f;
+  return q - floorf(q);
+}
+// p' = Exp(tau w) p + tau t, tau = s - s_ref: Rodrigues with a = sin(th) / th, b = (1 - cos(th)) / th^2 = 2 sin^2(th/2) / th^2
+// (no cancellation at small angles). tau == 0: the point's bits pass through (a -0 stays -0).
+SB_HD V3 deskew_point(V3 p, float tau, V3 w, V3 t) {
+  if (tau == 0.0f) return p;
+  const V3 wt = scale3(tau, w);
+  const float th2 = dot3(wt, wt);
+  float a = 1.0f, b = 0.5f;
+  if (th2 > 1e-30f) {
+    const float th = sqrtf(th2);
+    const float h = sinf_(0.5f * th);
+    a = sinf_(th) / th;
+    b = (2.0f * (h * h)) / th2;
+  }
+  const V3 c1 = cross3(wt, p);
+  const V3 c2 = cross3(wt, c1);
+  return mk3(((p.x + a * c1.x) + b * c2.x) + tau * t.x, ((p.y + a * c1.y) + b * c2.y) + tau * t.y,
+             ((p.z + a * c1.z) + b * c2.z) + tau * t.z);
+}
+
 // movable classes (color_map.glsl:8-17): car, bicycle, bus, motorcycle, truck, other-vehicle, person, bicyclist,
 // motorcyclist
 SB_HD bool is_movable(float l) {

@@ -12,12 +12,24 @@
 namespace sb {
 using namespace sbm;
 
-// K1a: gen_vertexmap.vert:73-91 -- one thread per point, scatter-min into the key image
+// K1a: gen_vertexmap.vert:73-91 -- one thread per point, scatter-min into the key image.
+// kDeskew: the point is first moved to the scan's reference time (DESIGN.md section 11) and written to dk.out, from where
+// k_preprocess_tile reads the winners; the off instance does not touch dk.
+template <bool kDeskew>
 __global__ void __launch_bounds__(256) k_project_scatter(KParams kp, const float4* __restrict__ pts, uint32_t n,
-                                                         unsigned long long* __restrict__ keys) {
+                                                         unsigned long long* __restrict__ keys, DeskewArgs dk) {
   uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   float4 p4 = __ldg(pts + i);
+  if (kDeskew) {
+    const float s = deskew_sweep_time(dk.mode, dk.mode == 1 ? __ldg(dk.times + i) : 0.0f,
+                                      dk.mode == 2 ? atan2f_(p4.y, p4.x) : 0.0f, dk.ref_time, dk.start_azimuth,
+                                      dk.clockwise);
+    const V3 q = deskew_point(mk3(p4.x, p4.y, p4.z), s - dk.ref_time, mk3(dk.w[0], dk.w[1], dk.w[2]),
+                              mk3(dk.t[0], dk.t[1], dk.t[2]));
+    p4 = make_float4(q.x, q.y, q.z, p4.w);
+    dk.out[i] = p4;
+  }
   V3 pos = mk3(p4.x, p4.y, p4.z);
   float d = len3(pos);
   float yaw = atan2f_(pos.y, pos.x);
@@ -276,14 +288,19 @@ size_t preprocess_key_elems(int W, int H) { return (size_t)(W + 2 * kPrepHalo) *
 
 void launch_preprocess(const Launch& L, const KParams& kp, const float4* pts, const float* labels, const float* probs,
                        uint32_t n, uint32_t timestamp, PrepKeys& keys, FrameDev out, float4* radius_map,
-                       unsigned long long* index_keys, uint8_t* integrated, uint32_t* group_counts) {
+                       unsigned long long* index_keys, uint8_t* integrated, uint32_t* group_counts,
+                       const DeskewArgs* deskew) {
   unsigned long long* cur = keys.img[keys.cur];
   unsigned long long* nxt = keys.img[keys.cur ^ 1];
   if (n > 0) {
     {
       ScopedKernel sk(L, K_PROJECT_SCATTER);
-      k_project_scatter<<<(n + 255) / 256, 256, 0, L.stream>>>(kp, pts, n, cur);
+      if (deskew)
+        k_project_scatter<true><<<(n + 255) / 256, 256, 0, L.stream>>>(kp, pts, n, cur, *deskew);
+      else
+        k_project_scatter<false><<<(n + 255) / 256, 256, 0, L.stream>>>(kp, pts, n, cur, DeskewArgs{});
     }
+    if (deskew) pts = deskew->out;  // the tile pass resolves the winners from the deskewed points
   }
   PrepIO io{pts, labels, probs, n, timestamp < 10 ? 1 : 0, cur, nxt, out.vertex, out.normal, out.semantic, radius_map,
             index_keys, integrated, group_counts};

@@ -83,14 +83,16 @@ TILE_POOL_SURFELS = 16 * 1024 * 1024  # the HBM share of a managed tile cache: t
 
 
 def run_sequence(seq_dir, params, make_engine=None, semantic=False, max_scans=None, on_scan=None, save_state=None,
-                 save_every=None, resume=None, tile_cache_host=0):
+                 save_every=None, resume=None, tile_cache_host=0, deskew="off"):
     """-> dict(poses=[4x4 float64 in the velodyne frame, from scan 0], seconds, scans processed by this call, and
     tile_cache: the cache's counters when tile_cache_host is set).
     `make_engine(params)` must return an object with processScan(points4, labels, probs) and getCurrentPose() -- the
     SurfelMapping surface -- and, for save_state / resume, save_state(), load_state(bytes) and timestamp(); for
     tile_cache_host, setTileCache(pool, host) and tile_cache_info().
     resume: a checkpoint written by save_state; the run continues at the scan after it (with the cache it was saved with).
-    tile_cache_host: surfels the managed tile cache may keep in host memory (inf: no bound; 0: the default cache)."""
+    tile_cache_host: surfels the managed tile cache may keep in host memory (inf: no bound; 0: the default cache).
+    deskew: "off" or "azimuth" (per-point deskewing by each point's azimuth, setDeskew); a resumed run keeps the setting
+    of its checkpoint."""
     files = list_scans(seq_dir)
     if max_scans is not None:
         files = files[:max_scans]
@@ -99,6 +101,8 @@ def run_sequence(seq_dir, params, make_engine=None, semantic=False, max_scans=No
     engine = (make_engine or _cuda_engine)(params)
     if tile_cache_host:
         engine.setTileCache(TILE_POOL_SURFELS, tile_cache_host)
+    if deskew != "off":
+        engine.setDeskew(deskew)
     poses = read_checkpoint(engine, resume) if resume else []
     first = len(poses)
     if first > len(files):
@@ -183,6 +187,9 @@ def main(argv=None, make_engine=None):
     ap.add_argument("--resume", default=None, metavar="PATH", help="continue from a --save-state checkpoint")
     ap.add_argument("--tile-cache-host", type=parse_host_surfels, default=0, metavar="N",
                     help="managed submap tile cache with up to N surfels in host memory (inf: no bound; 0: default cache)")
+    ap.add_argument("--deskew", choices=("off", "azimuth"), default="off",
+                    help="per-point deskewing by azimuth (off for KITTI odometry, whose scans are treated as already "
+                         "motion-compensated)")
     args = ap.parse_args(argv)
     if args.save_every is not None and (args.save_every <= 0 or not args.save_state):
         ap.error("--save-every needs --save-state and N > 0")
@@ -197,7 +204,7 @@ def main(argv=None, make_engine=None):
     params = api.default_params(data_width=args.width, model_width=args.width)
     res = run_sequence(args.seq, params, make_engine=make_engine, semantic=args.semantic, max_scans=args.max_scans,
                        save_state=args.save_state, save_every=args.save_every, resume=args.resume,
-                       tile_cache_host=args.tile_cache_host)
+                       tile_cache_host=args.tile_cache_host, deskew=args.deskew)
     calib_file = os.path.join(args.seq, "calib.txt")
     Tr = kitti.read_calibration(calib_file).get("Tr") if os.path.exists(calib_file) else None
     if args.out:

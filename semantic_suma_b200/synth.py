@@ -40,6 +40,26 @@ def rot_z(a):
     return np.array([[c, -s, 0, 0], [s, c, 0, 0], [0, 0, 1, 0], [0, 0, 0, 1]], np.float64)
 
 
+def so3_log(R):
+    """axis-angle of a rotation matrix (fp64)"""
+    v = np.array([R[2, 1] - R[1, 2], R[0, 2] - R[2, 0], R[1, 0] - R[0, 1]])
+    sv = np.linalg.norm(v)
+    return np.zeros(3) if sv == 0.0 else np.arctan2(0.5 * sv, 0.5 * (np.trace(R) - 1.0)) / sv * v
+
+
+def so3_exp(w):
+    """rotation matrices of axis-angle vectors w[..., 3] (Rodrigues, fp64)"""
+    w = np.asarray(w, np.float64)
+    th = np.linalg.norm(w, axis=-1)[..., None, None]
+    K = np.zeros(w.shape[:-1] + (3, 3))
+    K[..., 0, 1], K[..., 0, 2], K[..., 1, 2] = -w[..., 2], w[..., 1], -w[..., 0]
+    K[..., 1, 0], K[..., 2, 0], K[..., 2, 1] = w[..., 2], -w[..., 1], w[..., 0]
+    with np.errstate(divide="ignore", invalid="ignore"):
+        a = np.where(th > 0, np.sin(th) / th, 1.0)
+        b = np.where(th > 0, (1.0 - np.cos(th)) / (th * th), 0.5)
+    return np.eye(3) + a * K + b * (K @ K)
+
+
 def translate(x, y, z):
     T = np.eye(4)
     T[:3, 3] = (x, y, z)
@@ -73,9 +93,15 @@ class Scene:
         self.daz = 2.0 * np.pi / width
         self.delv = np.deg2rad(fov) / height
 
-    def scan(self, frame, pose=None):
+    def scan(self, frame, pose=None, rolling=None, ref_time=0.5):
         """Returns (pts[N,4] float32 (x,y,z,1) in the sensor frame, labels[N] float32, probs[N] float32).
-        Point order: azimuth-major, beams inner (as io/SimulationReader.cpp:103-116 builds its beam table)."""
+        Point order: azimuth-major, beams inner (as io/SimulationReader.cpp:103-116 builds its beam table).
+
+        rolling (a 4x4 per-frame increment, the sensor's true motion over one sweep): a rolling-shutter scan. Column k
+        is measured at sweep time s_k = (k + 0.5) / W (column 0 first, as a clockwise spin starting at yaw +pi) from
+        pose . D(s_k), D(s) = (Exp((s - ref_time) w), (s - ref_time) t) with (w, t) = (log R, t) of the increment; the
+        points come back in that instantaneous sensor frame and a fourth array holds their s_k. The same seed gives the
+        same noise and, with rolling=None, exactly the output of a plain scan."""
         rng = np.random.default_rng(self.seed + frame)
         if pose is None:
             pose = trajectory(frame + 1)[-1]
@@ -84,18 +110,30 @@ class Scene:
         el = np.tile(self.el, W) + rng.normal(0, self.jit, W * H) * self.delv
         ds = np.stack([np.cos(el) * np.cos(az), np.cos(el) * np.sin(az), np.sin(el)], 1)
         R, o = pose[:3, :3], pose[:3, 3]
-        d = ds @ R.T
+        margin = 0.0
+        if rolling is None:
+            d = ds @ R.T
+        else:
+            times = np.repeat((np.arange(W) + 0.5) / W, H)
+            tau = times - ref_time
+            w, t = so3_log(np.asarray(rolling)[:3, :3]), np.asarray(rolling)[:3, 3]
+            Rk = R @ so3_exp(tau[:, None] * w)           # world <- instantaneous sensor, per point
+            d = np.einsum("nij,nj->ni", Rk, ds)
+            o_center = o
+            o = o + (tau[:, None] * t) @ R.T
+            margin = float(np.linalg.norm(t))
+        o_c = o if rolling is None else o_center
         t_best = np.full(W * H, np.inf)
         hit = np.full(W * H, -1, np.int32)  # -1 none, 0 ground, 1+b box b
         with np.errstate(divide="ignore", invalid="ignore"):
-            tg = -o[2] / d[:, 2]
+            tg = -o[..., 2] / d[:, 2]
         m = (d[:, 2] < 0) & (tg > 0)
         t_best[m] = tg[m]
         hit[m] = 0
         for b, (bx, by, bz, yaw, size) in enumerate(_BOXES):
             if b in _MOVING:
                 bx = bx + 0.5 * frame
-            if (bx - o[0]) ** 2 + (by - o[1]) ** 2 > (self.max_range + size) ** 2:
+            if (bx - o_c[0]) ** 2 + (by - o_c[1]) ** 2 > (self.max_range + size + margin) ** 2:
                 continue
             Rb = rot_z(np.deg2rad(yaw))[:3, :3]
             ob = (o - np.array([bx, by, bz])) @ Rb
@@ -113,8 +151,9 @@ class Scene:
         keep = (hit >= 0) & (rngs >= self.min_range) & (rngs < self.max_range) & np.isfinite(rngs)
         pts = np.ones((int(keep.sum()), 4), np.float32)
         pts[:, :3] = (ds[keep] * rngs[keep, None]).astype(np.float32)
+        extra = () if rolling is None else (times[keep].astype(np.float32),)
         if not self.semantic:
-            return pts, None, None
+            return (pts, None, None) + extra
         hk = hit[keep]
         labels = np.where(hk == 0, 40.0, 50.0).astype(np.float32)
         for b in _CAR_BOXES:
@@ -122,7 +161,7 @@ class Scene:
         flips = rng.random(labels.shape[0]) < 0.02
         labels[flips] = rng.choice(np.array([10.0, 40.0, 50.0, 70.0, 30.0], np.float32), int(flips.sum()))
         probs = rng.uniform(0.6, 1.0, labels.shape[0]).astype(np.float32)
-        return pts, labels, probs
+        return (pts, labels, probs) + extra
 
 
 def make_sequence(n_frames, **kw):
