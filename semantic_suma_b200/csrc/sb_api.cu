@@ -28,16 +28,64 @@ struct sb_frame {
 };
 using FramePtr = Owned<sb_frame, std::default_delete<sb_frame>>;
 
-struct DevTile {  // SubmapCache, SurfelMap.h:179-181 -- kept in HBM (tile pool) instead of host RAM
-  uint32_t slot = 0;
-  bool known = false;  // base / count read back from the device record
-  uint32_t base = 0, count = 0;
+using TileKey = std::pair<int32_t, int32_t>;  // submap tile index (i, j)
+
+// The tile pool's records, {end in the pool, surfels of the tile} per slot: slot s holds [end of slot s - 1, end of s).
+struct TileRecords {
+  std::vector<uint2> v;
+  uint32_t base(uint32_t s) const { return s ? v[s - 1].x : 0u; }
+  uint32_t size(uint32_t s) const { return v[s].x - base(s); }
+  uint32_t end() const { return v.empty() ? 0u : v.back().x; }
+  uint64_t dropped() const {  // surfels of these extractions that did not fit the pool (the extract cap is no drop)
+    uint64_t n = 0;
+    for (uint32_t s = 0; s < v.size(); ++s) n += std::min(v[s].y, kExtractCap) - size(s);
+    return n;
+  }
 };
 
 // A tile of the managed cache's host tier: its surfels as four lanes of pitch `count` in a pinned buffer of `cap` surfels
 struct HostTile {
   uint32_t count = 0, cap = 0;
   PinnedPtr<float4> buf;
+};
+
+// Submap paging (SurfelMap.cpp:744-824) and its tile cache, in an HBM pool and a host tier (DESIGN.md section 10).
+struct Paging {
+  struct Setting {
+    bool managed = false;              // off by default, and then the host tier, reclaim and eviction are never used
+    uint32_t pool_cap = kTilePoolCap;  // HBM share (the pool allocation stays kTilePoolCap)
+    uint64_t host_cap = 0;             // surfels the host tier may hold
+  };
+  struct Counters {  // dropped_retired: drops counted on record slots that a reclaim has since renumbered
+    uint64_t reclaims = 0, reclaim_moved = 0, evictions = 0, host_fills = 0, dropped_retired = 0;
+  };
+  int32_t origin_i = 0, origin_j = 0;  // the active window's centre tile
+  std::vector<TileKey> extraction;     // tiles that left the window and are still to be extracted
+  SurfelPlanes pool{};                 // tile pool lanes
+  DevPtr<float4> pool_mem;
+  DevPtr<uint2> d_rec;                 // the records of slots [0, n_slots), written by the extractions
+  uint32_t n_slots = 0;
+  TileRecords rec;  // host copy of the records of slots [0, n_known): a tile is known when its slot is below n_known
+  std::map<TileKey, uint32_t> tiles;   // pool tiles and their slots
+  std::map<TileKey, HostTile> host;    // host-tier tiles (never also in `tiles`)
+  uint64_t host_used = 0;
+  std::multimap<uint32_t, PinnedPtr<float4>> spare;  // pinned buffers of replaced host tiles, by capacity
+  Setting setting;
+  uint64_t pool_bound = 0;             // upper bound of the pool's used end that the host has without a read-back
+  Counters counters;
+  DevPtr<uint2> segs;                  // move list of a reclaim
+
+  uint32_t n_known() const { return (uint32_t)rec.v.size(); }
+  bool known(uint32_t slot) const { return slot < n_known(); }
+  bool pending() const { return n_known() < n_slots; }  // some records have not been read back yet
+  bool empty() const { return n_slots == 0 && tiles.empty() && host.empty(); }
+  // A host tile gives its pinned buffer back for reuse (the copies that read it are ordered on the stream).
+  void release(HostTile& h) { host_used -= h.count; if (h.buf) spare.emplace(h.cap, std::move(h.buf)); }
+  void clear() {  // empties the window and both tiers (SurfelMap::reset) and keeps the setting
+    for (auto& kv : host) release(kv.second);
+    host.clear(); tiles.clear(); extraction.clear(); rec.v.clear();
+    origin_i = origin_j = 0; n_slots = 0; pool_bound = 0; counters = Counters{};
+  }
 };
 
 struct sb_ctx {
@@ -137,27 +185,7 @@ struct sb_ctx {
   // one past the largest pose-table entry a surfel of the map or of a cached tile can refer to (creation timestamp,
   // clamped as pose_index() does): while it is <= map_timestamp, no surfel reads the entry the scan's pose goes into
   uint32_t pose_ref_end = 0;
-  int32_t origin_i = 0, origin_j = 0;
-  std::vector<std::pair<int32_t, int32_t>> extraction;
-  std::map<std::pair<int32_t, int32_t>, DevTile> tiles;
-  SurfelPlanes pool{};            // tile cache lanes
-  DevPtr<float4> pool_mem;
-  DevPtr<uint2> d_tile_rec;       // {end in the pool, surfels of the tile} per extraction; slot s starts at the end of s - 1
-  uint32_t n_slots = 0;
-  bool tiles_pending = false;     // some records have not been read back yet
-  // managed tile cache (sb_set_tile_cache; DESIGN.md section 10): off by default, and then none of this is touched
-  struct TileCache {
-    bool managed = false;
-    uint32_t pool_cap = kTilePoolCap;  // HBM share (the pool allocation stays kTilePoolCap)
-    uint64_t host_cap = 0;             // surfels the host tier may hold
-    uint64_t pool_bound = 0;           // upper bound of the pool's used end that the host has without a read-back
-    uint64_t host_used = 0;
-    uint64_t reclaims = 0, reclaim_moved = 0, evictions = 0, host_fills = 0;
-    uint64_t dropped_retired = 0;      // drops counted on record slots that a reclaim has since renumbered
-    std::map<std::pair<int32_t, int32_t>, HostTile> host;  // host-resident tiles (never also in `tiles`)
-    std::multimap<uint32_t, PinnedPtr<float4>> spare;       // pinned buffers of replaced host tiles, by capacity
-    DevPtr<uint2> segs;                // move list of a reclaim
-  } tc;
+  Paging pg;
 
   // Full-render memo: SurfelMapping re-renders the unchanged map at the unchanged pose at the start of the next scan
   // (SurfelMapping.cpp:351 after :803); identical arguments on an unmodified map reproduce identical images. The memo
@@ -305,27 +333,24 @@ void frame_written(sb_ctx* c, const sb_frame* f) {
   if (f == c->f_old || f == c->f_new || f == c->f_comp || f->id == c->memo.key.out) c->memo.clear();
 }
 
-// The host tier's tiles give their pinned buffers back for reuse (the copies that read them are ordered on the stream).
-void release_host_tile(sb_ctx* c, HostTile& h) {
-  c->tc.host_used -= h.count;
-  if (h.buf) c->tc.spare.emplace(h.cap, std::move(h.buf));
-}
-
-// A pinned buffer of at least h.count surfels for a host tile: a spare one when one is large enough, else a new one.
-int acquire_host_buffer(sb_ctx* c, HostTile& h) {
-  if (h.count == 0) return SB_OK;
-  auto sp = c->tc.spare.lower_bound(h.count);
-  if (sp != c->tc.spare.end()) {
+// A new host-tier tile of `count` surfels; its pinned buffer is a spare one when one is large enough, else a new one.
+int add_host_tile(sb_ctx* c, const TileKey& idx, uint32_t count, HostTile** out) {
+  Paging& pg = c->pg;
+  HostTile h;
+  h.count = h.cap = count;
+  auto sp = pg.spare.lower_bound(count);
+  if (count && sp != pg.spare.end()) {
     h.cap = sp->first;
     h.buf = std::move(sp->second);
-    c->tc.spare.erase(sp);
-    return SB_OK;
+    pg.spare.erase(sp);
+  } else if (count) {
+    void* p = nullptr;
+    cudaError_t e = cudaMallocHost(&p, (size_t)count * 64);
+    if (e != cudaSuccess) return fail(c, SB_ERR_NOMEM, std::string("tile cache host tier: ") + cudaGetErrorString(e));
+    h.buf.reset(static_cast<float4*>(p));
   }
-  void* p = nullptr;
-  cudaError_t e = cudaMallocHost(&p, (size_t)h.count * 64);
-  if (e != cudaSuccess) return fail(c, SB_ERR_NOMEM, std::string("tile cache host tier: ") + cudaGetErrorString(e));
-  h.cap = h.count;
-  h.buf.reset(static_cast<float4*>(p));
+  pg.host_used += count;
+  *out = &(pg.host[idx] = std::move(h));
   return SB_OK;
 }
 
@@ -334,15 +359,7 @@ int reset_state(sb_ctx* c) {
   c->map_version += 1;
   c->n_host = 0; c->n_holes = 0; c->lazy_update = false;
   c->n_updated = 0; c->n_new = 0; c->map_timestamp = 0; c->pose_ref_end = 0;
-  c->origin_i = c->origin_j = 0;
-  c->extraction.clear();
-  c->tiles.clear();
-  c->n_slots = 0;
-  c->tiles_pending = false;
-  for (auto& kv : c->tc.host) release_host_tile(c, kv.second);
-  c->tc.host.clear();
-  c->tc.pool_bound = 0;
-  c->tc.reclaims = c->tc.reclaim_moved = c->tc.evictions = c->tc.host_fills = c->tc.dropped_retired = 0;
+  c->pg.clear();
   c->stats[12] = 0.0;
   c->loop.reset();  // posegraph_->clear(); trajectory_distances_ ... (SurfelMapping.cpp:158-163)
   for (int i = 0; i < 16; ++i) c->lastPose_old[i] = (i % 5 == 0) ? 1.0 : 0.0;
@@ -411,8 +428,8 @@ int alloc_buffers(sb_ctx* c) {
   if ((r = alloc_planes(c, c->T_mem, &c->T, kMaxSurfels))) return r;
   if ((r = alloc_planes(c, c->G_mem, &c->G, Pd))) return r;
   if ((r = alloc_planes(c, c->X_mem, &c->X, 16))) return r;
-  if ((r = alloc_planes(c, c->pool_mem, &c->pool, kTilePoolCap))) return r;
-  SB_CUDA(c, dev_alloc(c->d_tile_rec, (size_t)kMaxTileSlots * sizeof(uint2)));
+  if ((r = alloc_planes(c, c->pg.pool_mem, &c->pg.pool, kTilePoolCap))) return r;
+  SB_CUDA(c, dev_alloc(c->pg.d_rec, (size_t)kMaxTileSlots * sizeof(uint2)));
   SB_CUDA(c, dev_alloc(c->live, kMaxSurfels));
   SB_CUDA(c, dev_alloc(c->keep, kMaxSurfels));
   size_t nb = (kMaxSurfels + 127) / 128 + 16;  // blocks of the finest-grained surfel kernel
@@ -725,40 +742,6 @@ int fetch_counts(sb_ctx* c, uint32_t* dst, int n) {
   return SB_OK;
 }
 
-// read back the records of the tiles extracted so far (all of them into *out, if given, even when none is pending)
-int refresh_tile_records(sb_ctx* c, std::vector<uint2>* out = nullptr) {
-  if (out) out->clear();
-  if ((!c->tiles_pending && !out) || c->n_slots == 0) return SB_OK;
-  std::vector<uint2> local;
-  std::vector<uint2>& rec = out ? *out : local;
-  rec.resize(c->n_slots);
-  SB_CUDA(c, cudaMemcpyAsync(rec.data(), c->d_tile_rec, (size_t)c->n_slots * sizeof(uint2), cudaMemcpyDeviceToHost,
-                             c->stream));
-  SB_CUDA(c, cudaStreamSynchronize(c->stream));
-  auto base = [&](uint32_t s) { return s ? rec[s - 1].x : 0u; };
-  {  // surfels that did not fit the 16 M-surfel HBM tile pool (the reference's host-side cache is unbounded); slots are
-     // never reused, so the sum over all slots counts every drop since the last reset (a managed cache renumbers them
-     // and carries the drops of the retired slots in dropped_retired)
-    uint64_t dropped = c->tc.dropped_retired;
-    for (uint32_t s = 0; s < c->n_slots; ++s) dropped += std::min(rec[s].y, kExtractCap) - (rec[s].x - base(s));
-    if ((double)dropped != c->stats[12]) {
-      c->stats[12] = (double)dropped;
-      c->err = "submap tile pool exhausted: " + std::to_string(dropped) + " surfels of leaving tiles were dropped";
-    }
-  }
-  for (auto& kv : c->tiles) {
-    DevTile& t = kv.second;
-    if (!t.known) {
-      t.base = base(t.slot);
-      t.count = rec[t.slot].x - t.base;
-      t.known = true;
-    }
-  }
-  c->tiles_pending = false;
-  c->tc.pool_bound = c->n_slots ? rec[c->n_slots - 1].x : 0u;
-  return SB_OK;
-}
-
 // Moves the live surfels of a map with dead slots to the front, in order (A -> T, then the two sets swap roles): what
 // observers of the map and the operator-level update see, and what a tile that needs the room finds.
 int compact_map(sb_ctx* c) {
@@ -779,22 +762,57 @@ int compact_map(sb_ctx* c) {
   return SB_OK;
 }
 
+// ---- submap paging and its tile cache (DESIGN.md section 10) ----
+// The window the map update keeps (SurfelMap.cpp:674-677): its extent, and its centre into *ctr.
+float active_window(const sb_ctx* c, float2* ctr) {
+  *ctr = submap_center(c, c->pg.origin_i, c->pg.origin_j);
+  const float extent = 2.0f * c->p.submap_dimension * c->p.submap_extent + c->p.submap_extent;
+  return c->p.partial_extraction && !c->pg.extraction.empty() ? extent + 2.0f * c->p.submap_extent : extent;
+}
+
+// The records of slots [0, n_slots) as the device holds them (one synchronisation when there are any).
+int read_tile_records(sb_ctx* c, TileRecords& o) {
+  o.v.resize(c->pg.n_slots);
+  if (o.v.empty()) return SB_OK;
+  SB_CUDA(c, cudaMemcpyAsync(o.v.data(), c->pg.d_rec, o.v.size() * sizeof(uint2), cudaMemcpyDeviceToHost, c->stream));
+  SB_CUDA(c, cudaStreamSynchronize(c->stream));
+  return SB_OK;
+}
+
+// Reads the records back when some are pending (or `always`), so that every tile is known.
+int refresh_tile_records(sb_ctx* c, bool always = false) {
+  Paging& pg = c->pg;
+  if ((!always && !pg.pending()) || pg.n_slots == 0) return SB_OK;
+  if (int r = read_tile_records(c, pg.rec)) return r;
+  // surfels that did not fit the 16 M-surfel HBM tile pool (the reference's host-side cache is unbounded); slots are
+  // never reused, so the sum over all slots counts every drop since the last reset (a managed cache renumbers them and
+  // carries the drops of the retired slots in dropped_retired)
+  const uint64_t dropped = pg.counters.dropped_retired + pg.rec.dropped();
+  if ((double)dropped != c->stats[12]) {
+    c->stats[12] = (double)dropped;
+    c->err = "submap tile pool exhausted: " + std::to_string(dropped) + " surfels of leaving tiles were dropped";
+  }
+  pg.pool_bound = pg.rec.end();
+  return SB_OK;
+}
+
 int append_tiles(sb_ctx* c, int32_t i0, int32_t j0, int di, int dj) {  // SurfelMap.cpp:769-780
+  Paging& pg = c->pg;
   const int dim = c->p.submap_dimension;
   int r;
   bool appended = false;
   for (int32_t k = -dim; k <= dim; ++k) {
-    const std::pair<int32_t, int32_t> idx(i0 + di * k, j0 + dj * k);
-    auto it = c->tiles.find(idx);
+    const TileKey idx(i0 + di * k, j0 + dj * k);
+    auto it = pg.tiles.find(idx);
     const HostTile* h = nullptr;
-    if (it == c->tiles.end()) {
-      auto hi = c->tc.host.find(idx);
-      if (hi == c->tc.host.end()) continue;  // submapCache_[idx] of a tile never extracted: empty
+    if (it == pg.tiles.end()) {
+      auto hi = pg.host.find(idx);
+      if (hi == pg.host.end()) continue;  // submapCache_[idx] of a tile never extracted: empty
       h = &hi->second;  // a tile of the managed cache's host tier: it stays there until it is extracted again
-    } else if (!it->second.known && (r = refresh_tile_records(c))) {
+    } else if (!pg.known(it->second) && (r = refresh_tile_records(c))) {
       return r;
     }
-    const uint32_t count = h ? h->count : it->second.count;
+    const uint32_t count = h ? h->count : pg.rec.size(it->second);
     // the reference's map has no dead slots: a tile that does not fit behind them fits (or is cut) after compaction
     if (count > kMaxSurfels - c->n_host && (r = compact_map(c))) return r;
     uint32_t room = kMaxSurfels - c->n_host;
@@ -808,10 +826,10 @@ int append_tiles(sb_ctx* c, int32_t i0, int32_t j0, int di, int dj) {  // Surfel
                                    cudaMemcpyHostToDevice, c->stream));
       else
         SB_CUDA(c, cudaMemcpyAsync(c->A.p0 + lane * kMaxSurfels + c->n_host,
-                                   c->pool.p0 + lane * kTilePoolCap + it->second.base, (size_t)n * 16,
+                                   pg.pool.p0 + lane * kTilePoolCap + pg.rec.base(it->second), (size_t)n * 16,
                                    cudaMemcpyDeviceToDevice, c->stream));
     }
-    if (h) c->tc.host_fills += 1;
+    if (h) pg.counters.host_fills += 1;
     SB_CUDA(c, cudaMemsetAsync(c->live + c->n_host, 1, n, c->stream));
     c->n_host += n;
     c->n_upper = c->n_host;
@@ -825,42 +843,39 @@ int append_tiles(sb_ctx* c, int32_t i0, int32_t j0, int di, int dj) {  // Surfel
   return SB_OK;
 }
 
-// ---- managed tile cache (DESIGN.md section 10) ----
-// Compacts the pool: the ranges of the cached tiles move to its front in pool order (through the idle scratch set T, in
-// rounds of at most kMaxSurfels, so that no range is read after it has been overwritten), their records become dense
-// again and their slots are renumbered 0 .. tiles - 1. rec: the records as on the device (every tile is known); updated.
-int reclaim_pool(sb_ctx* c, std::vector<uint2>& rec) {
-  sb_ctx::TileCache& tc = c->tc;
-  std::vector<DevTile*> order;
-  for (auto& kv : c->tiles) order.push_back(&kv.second);
-  std::sort(order.begin(), order.end(), [](const DevTile* a, const DevTile* b) { return a->slot < b->slot; });
-  const uint32_t end = c->n_slots ? rec[c->n_slots - 1].x : 0u;
+// Compacts the managed cache's pool: the ranges of the cached tiles move to its front in pool order (through the idle
+// scratch set T, in rounds of at most kMaxSurfels, so that no range is read after it has been overwritten), their
+// records become dense again and their slots are renumbered 0 .. tiles - 1. Every tile is known.
+int reclaim_pool(sb_ctx* c) {
+  Paging& pg = c->pg;
+  std::vector<uint32_t*> order;  // the tiles' slots, in pool order
+  for (auto& kv : pg.tiles) order.push_back(&kv.second);
+  std::sort(order.begin(), order.end(), [](const uint32_t* a, const uint32_t* b) { return *a < *b; });
+  const uint32_t end = pg.rec.end();
   uint64_t referenced = 0;
-  for (const DevTile* t : order) referenced += t->count;
-  if (referenced == end && order.size() == c->n_slots) {
-    tc.pool_bound = end;
+  for (const uint32_t* s : order) referenced += pg.rec.size(*s);
+  if (referenced == end && order.size() == pg.n_slots) {
+    pg.pool_bound = end;
     return SB_OK;
   }
-  // the drops of the slots that go away stay counted
-  for (uint32_t s = 0; s < c->n_slots; ++s)
-    tc.dropped_retired += std::min(rec[s].y, kExtractCap) - (rec[s].x - (s ? rec[s - 1].x : 0u));
+  pg.counters.dropped_retired += pg.rec.dropped();  // the drops of the slots that go away stay counted
   // moves in pool order: (source, destination) runs of adjacent tiles; the tiles already in place stay
   struct Run { uint32_t src, dst, n; };
   std::vector<Run> runs;
-  std::vector<uint2> nrec(order.size());
+  TileRecords nrec{std::vector<uint2>(order.size())};
   uint32_t dst = 0;
   for (size_t k = 0; k < order.size(); ++k) {
-    DevTile& t = *order[k];
-    if (t.count && t.base != dst) {
-      if (!runs.empty() && runs.back().src + runs.back().n == t.base && runs.back().dst + runs.back().n == dst)
-        runs.back().n += t.count;
+    uint32_t& slot = *order[k];
+    const uint32_t base = pg.rec.base(slot), count = pg.rec.size(slot);
+    if (count && base != dst) {
+      if (!runs.empty() && runs.back().src + runs.back().n == base && runs.back().dst + runs.back().n == dst)
+        runs.back().n += count;
       else
-        runs.push_back(Run{t.base, dst, t.count});
+        runs.push_back(Run{base, dst, count});
     }
-    t.slot = (uint32_t)k;
-    t.base = dst;
-    dst += t.count;
-    nrec[k] = make_uint2(dst, t.count);
+    slot = (uint32_t)k;
+    dst += count;
+    nrec.v[k] = make_uint2(dst, count);
   }
   // rounds: each gathers up to kMaxSurfels of the moved surfels into T and writes them back to their destination; a
   // destination lies at or below its source, and the sources of later rounds lie above this round's destinations
@@ -882,43 +897,37 @@ int reclaim_pool(sb_ctx* c, std::vector<uint2>& rec) {
       o += n;
     }
   if (!segs.empty()) {
-    if (!tc.segs) SB_CUDA(c, dev_alloc(tc.segs, ((size_t)kMaxTileSlots + 64) * sizeof(uint2)));
-    SB_CUDA(c, cudaMemcpyAsync(tc.segs, segs.data(), segs.size() * sizeof(uint2), cudaMemcpyHostToDevice, c->stream));
+    if (!pg.segs) SB_CUDA(c, dev_alloc(pg.segs, ((size_t)kMaxTileSlots + 64) * sizeof(uint2)));
+    SB_CUDA(c, cudaMemcpyAsync(pg.segs, segs.data(), segs.size() * sizeof(uint2), cudaMemcpyHostToDevice, c->stream));
     Launch L = L_(c);
     for (size_t q = 0; q < round_n.size(); ++q) {
       const uint32_t s0 = seg_begin[q], s1 = q + 1 < round_n.size() ? seg_begin[q + 1] : (uint32_t)segs.size();
-      launch_pool_reclaim(L, c->pool, c->T, tc.segs + s0, s1 - s0, 0, 0, round_n[q]);
-      launch_pool_reclaim(L, c->T, c->pool, nullptr, 0, 0, round_dst[q], round_n[q]);
+      launch_pool_reclaim(L, pg.pool, c->T, pg.segs + s0, s1 - s0, 0, 0, round_n[q]);
+      launch_pool_reclaim(L, c->T, pg.pool, nullptr, 0, 0, round_dst[q], round_n[q]);
     }
   }
-  if (!nrec.empty())
-    SB_CUDA(c, cudaMemcpyAsync(c->d_tile_rec, nrec.data(), nrec.size() * sizeof(uint2), cudaMemcpyHostToDevice, c->stream));
+  if (!nrec.v.empty())
+    SB_CUDA(c, cudaMemcpyAsync(pg.d_rec, nrec.v.data(), nrec.v.size() * sizeof(uint2), cudaMemcpyHostToDevice, c->stream));
   SB_CUDA(c, cudaStreamSynchronize(c->stream));  // the copies read host vectors
-  rec = nrec;
-  c->n_slots = (uint32_t)order.size();
-  tc.pool_bound = dst;
-  tc.reclaims += 1;
-  for (uint32_t n : round_n) tc.reclaim_moved += n;
+  pg.rec = std::move(nrec);
+  pg.n_slots = (uint32_t)order.size();
+  pg.pool_bound = dst;
+  pg.counters.reclaims += 1;
+  for (uint32_t n : round_n) pg.counters.reclaim_moved += n;
   return SB_OK;
 }
 
-// Moves one pool tile to the host tier (its pool range is abandoned until the next reclaim).
-int evict_tile(sb_ctx* c, std::map<std::pair<int32_t, int32_t>, DevTile>::iterator it) {
-  sb_ctx::TileCache& tc = c->tc;
-  const DevTile& t = it->second;
-  HostTile h;
-  h.count = t.count;
-  int r;
-  if ((r = acquire_host_buffer(c, h))) return r;
-  if (t.count) {
-    for (size_t lane = 0; lane < 4; ++lane)
-      SB_CUDA(c, cudaMemcpyAsync(h.buf + lane * t.count, c->pool.p0 + lane * kTilePoolCap + t.base, (size_t)t.count * 16,
-                                 cudaMemcpyDeviceToHost, c->stream));
-  }
-  tc.host_used += t.count;
-  tc.evictions += 1;
-  tc.host[it->first] = std::move(h);
-  c->tiles.erase(it);
+// Moves one known pool tile to the host tier (its pool range is abandoned until the next reclaim).
+int evict_tile(sb_ctx* c, std::map<TileKey, uint32_t>::iterator it) {
+  Paging& pg = c->pg;
+  const uint32_t base = pg.rec.base(it->second), count = pg.rec.size(it->second);
+  HostTile* h;
+  if (int r = add_host_tile(c, it->first, count, &h)) return r;
+  for (size_t lane = 0; lane < 4 && count; ++lane)
+    SB_CUDA(c, cudaMemcpyAsync(h->buf + lane * count, pg.pool.p0 + lane * kTilePoolCap + base, (size_t)count * 16,
+                               cudaMemcpyDeviceToHost, c->stream));
+  pg.counters.evictions += 1;
+  pg.tiles.erase(it);
   return SB_OK;
 }
 
@@ -928,95 +937,90 @@ int evict_tile(sb_ctx* c, std::map<std::pair<int32_t, int32_t>, DevTile>::iterat
 // Eviction order: the tile farthest from the window origin (Chebyshev distance in tile indices) first, the oldest
 // extraction (lowest slot, the pool order) among equals -- replicated state only, so striped ranks stay identical.
 int make_tile_room(sb_ctx* c) {
-  sb_ctx::TileCache& tc = c->tc;
-  if (tc.pool_bound + kExtractCap <= tc.pool_cap && c->n_slots < kMaxTileSlots) return SB_OK;
-  std::vector<uint2> rec;
+  Paging& pg = c->pg;
+  if (pg.pool_bound + kExtractCap <= pg.setting.pool_cap && pg.n_slots < kMaxTileSlots) return SB_OK;
   int r;
-  if ((r = refresh_tile_records(c, &rec))) return r;
-  if ((r = reclaim_pool(c, rec))) return r;
-  const uint64_t need = tc.pool_bound + kExtractCap > tc.pool_cap ? tc.pool_bound + kExtractCap - tc.pool_cap : 0;
-  const uint32_t need_slots = c->n_slots >= kMaxTileSlots ? c->n_slots + 1 - kMaxTileSlots : 0;
+  if ((r = refresh_tile_records(c, true))) return r;
+  if ((r = reclaim_pool(c))) return r;
+  const uint64_t need = pg.pool_bound + kExtractCap > pg.setting.pool_cap ? pg.pool_bound + kExtractCap - pg.setting.pool_cap : 0;
+  const uint32_t need_slots = pg.n_slots >= kMaxTileSlots ? pg.n_slots + 1 - kMaxTileSlots : 0;
   if (need == 0 && need_slots == 0) return SB_OK;
-  using Key = std::pair<int32_t, int32_t>;
-  std::vector<std::pair<std::pair<int64_t, uint32_t>, Key>> cand;  // ((-distance, slot), tile)
-  for (const auto& kv : c->tiles) {
-    const int64_t d = std::max(std::llabs((long long)kv.first.first - c->origin_i),
-                               std::llabs((long long)kv.first.second - c->origin_j));
-    cand.push_back(std::make_pair(std::make_pair(-d, kv.second.slot), kv.first));
+  std::vector<std::pair<std::pair<int64_t, uint32_t>, TileKey>> cand;  // ((-distance, slot), tile)
+  for (const auto& kv : pg.tiles) {
+    const int64_t d = std::max(std::llabs((long long)kv.first.first - pg.origin_i),
+                               std::llabs((long long)kv.first.second - pg.origin_j));
+    cand.push_back(std::make_pair(std::make_pair(-d, kv.second), kv.first));
   }
   std::sort(cand.begin(), cand.end());
   uint64_t freed = 0;
   uint32_t freed_slots = 0;
   for (const auto& e : cand) {
     if (freed >= need && freed_slots >= need_slots) break;
-    auto it = c->tiles.find(e.second);
-    if (it->second.count == 0 && freed_slots >= need_slots) continue;  // an empty tile frees only a slot
-    if (tc.host_used + it->second.count > tc.host_cap) continue;       // does not fit the host tier
-    freed += it->second.count;
+    auto it = pg.tiles.find(e.second);
+    const uint32_t count = pg.rec.size(it->second);
+    if (count == 0 && freed_slots >= need_slots) continue;  // an empty tile frees only a slot
+    if (pg.host_used + count > pg.setting.host_cap) continue;  // does not fit the host tier
+    freed += count;
     freed_slots += 1;
     if ((r = evict_tile(c, it))) return r;
   }
   // (nothing moved: both tiers are full, and the extraction is cut as the default cache cuts it)
-  return freed_slots ? reclaim_pool(c, rec) : SB_OK;
+  return freed_slots ? reclaim_pool(c) : SB_OK;
 }
 
 // SurfelMap.cpp:708-742 + extract_surfels.vert: the tile is compacted into the HBM pool; nothing is read back here
 int extract_surfels(sb_ctx* c, bool partially) {
+  Paging& pg = c->pg;
   Launch L = L_(c);
   int r;
-  while (!c->extraction.empty()) {
-    std::pair<int32_t, int32_t> idx = c->extraction.back();
-    c->extraction.pop_back();
-    if (c->tc.managed) {
+  while (!pg.extraction.empty()) {
+    TileKey idx = pg.extraction.back();
+    pg.extraction.pop_back();
+    if (pg.setting.managed) {
       // the new extraction replaces the tile's cached copy: drop it first, so that a reclaim can use its pool range
-      c->tiles.erase(idx);
-      auto hi = c->tc.host.find(idx);
-      if (hi != c->tc.host.end()) {
-        release_host_tile(c, hi->second);
-        c->tc.host.erase(hi);
+      pg.tiles.erase(idx);
+      auto hi = pg.host.find(idx);
+      if (hi != pg.host.end()) {
+        pg.release(hi->second);
+        pg.host.erase(hi);
       }
       if ((r = make_tile_room(c))) return r;
-      c->tc.pool_bound += kExtractCap;
+      pg.pool_bound += kExtractCap;
     }
-    if (c->n_slots >= kMaxTileSlots) return fail(c, SB_ERR_CAPACITY, "tile cache: out of record slots");
+    if (pg.n_slots >= kMaxTileSlots) return fail(c, SB_ERR_CAPACITY, "tile cache: out of record slots");
     float2 ctr = submap_center(c, idx.first, idx.second);
-    uint32_t slot = c->n_slots++;
+    uint32_t slot = pg.n_slots++;
     // extractions can follow each other with no per-pixel prologue in between to clear the group totals
     SB_CUDA(c, cudaMemsetAsync(c->group_counts, 0, kGroupCounts * 4, c->stream));
     launch_extract_to_pool(L, c->A, c->res->counts, c->live, c->n_host, c->poses, ctr, c->p.submap_extent, c->keep,
-                           c->block_counts, c->group_counts, c->pool, c->tc.pool_cap, c->d_tile_rec, slot, kExtractCap);
-    DevTile t;
-    t.slot = slot;
-    t.known = false;
-    c->tiles[idx] = t;  // a tile extracted again replaces its cache entry (the old pool range is abandoned)
-    c->tiles_pending = true;
+                           c->block_counts, c->group_counts, pg.pool, pg.setting.pool_cap, pg.d_rec, slot, kExtractCap);
+    pg.tiles[idx] = slot;  // a tile extracted again replaces its cache entry (the old pool range is abandoned)
     if (partially) break;
   }
   return SB_OK;
 }
 
 int update_active_submaps(sb_ctx* c, const float* pose) {  // SurfelMap.cpp:744-824
+  Paging& pg = c->pg;
   const int dim = c->p.submap_dimension;
   const float ext = c->p.submap_extent;
-  float2 ctr = submap_center(c, c->origin_i, c->origin_j);
+  float2 ctr = submap_center(c, pg.origin_i, pg.origin_j);
   float changex = pose[12] - ctr.x, changey = pose[13] - ctr.y;
   float factor = 1.1f;
   int r;
-  if (fabsf(changex) > factor * ext || fabsf(changey) > factor * ext) {
-    if (fabsf(changex) > factor * ext) {
-      int dir = changex < 0 ? -1 : 1;
-      for (int32_t k = -dim; k <= dim; ++k) c->extraction.push_back(std::make_pair(c->origin_i - dir * dim, c->origin_j + k));
-      c->origin_i += dir;
-      if ((r = append_tiles(c, c->origin_i + dir * dim, c->origin_j, 0, 1))) return r;
-    }
-    if (fabsf(changey) > factor * ext) {
-      int dir = changey < 0 ? -1 : 1;
-      for (int32_t k = -dim; k <= dim; ++k) c->extraction.push_back(std::make_pair(c->origin_i + k, c->origin_j - dir * dim));
-      c->origin_j += dir;
-      if ((r = append_tiles(c, c->origin_i, c->origin_j + dir * dim, 1, 0))) return r;
-    }
+  if (fabsf(changex) > factor * ext) {
+    int dir = changex < 0 ? -1 : 1;
+    for (int32_t k = -dim; k <= dim; ++k) pg.extraction.push_back(TileKey(pg.origin_i - dir * dim, pg.origin_j + k));
+    pg.origin_i += dir;
+    if ((r = append_tiles(c, pg.origin_i + dir * dim, pg.origin_j, 0, 1))) return r;
   }
-  if (!c->extraction.empty()) return extract_surfels(c, c->p.partial_extraction != 0);
+  if (fabsf(changey) > factor * ext) {
+    int dir = changey < 0 ? -1 : 1;
+    for (int32_t k = -dim; k <= dim; ++k) pg.extraction.push_back(TileKey(pg.origin_i + k, pg.origin_j - dir * dim));
+    pg.origin_j += dir;
+    if ((r = append_tiles(c, pg.origin_i, pg.origin_j + dir * dim, 1, 0))) return r;
+  }
+  if (!pg.extraction.empty()) return extract_surfels(c, c->p.partial_extraction != 0);
   return SB_OK;
 }
 
@@ -1052,9 +1056,8 @@ int map_update(sb_ctx* c, const float* pose, const sb_frame* frame, const Mat4* 
   launch_index_scatter(L, kp, c->A, c->res->counts, c->live, n_grid(c), c->Mtab_old, c->key_index,
                        index_fused ? &c->res->pose.fallback : nullptr);
   // K6c + K6e predicate
-  float2 ctr = submap_center(c, c->origin_i, c->origin_j);
-  float extent = 2.0f * c->p.submap_dimension * c->p.submap_extent + c->p.submap_extent;  // :674
-  if (c->p.partial_extraction && !c->extraction.empty()) extent += 2.0f * c->p.submap_extent;  // :677
+  float2 ctr;
+  const float extent = active_window(c, &ctr);
   // In place (lazy) or dense, decided from what the host already knows (no extra synchronisation); DESIGN.md section 7.
   // Dense when the dead slots reach 1 / kDenseHoleFraction of the physical end, when the new surfels could hit the capacity
   // behind the dead slots (k_gen_compact must cut exactly where the compacted map would), and at the operator level.
@@ -1923,9 +1926,9 @@ int sb_map_update_debug(sb_ctx* c, uint32_t* index_map, float* radius_map4, uint
 }
 int sb_map_submap_origin(sb_ctx* c, int32_t* i, int32_t* j, uint32_t* pending) {
   if (!c) return SB_ERR_INVALID;
-  if (i) *i = c->origin_i;
-  if (j) *j = c->origin_j;
-  if (pending) *pending = (uint32_t)c->extraction.size();
+  if (i) *i = c->pg.origin_i;
+  if (j) *j = c->pg.origin_j;
+  if (pending) *pending = (uint32_t)c->pg.extraction.size();
   return SB_OK;
 }
 
@@ -1933,41 +1936,33 @@ int sb_set_tile_cache(sb_ctx* c, uint32_t pool_surfels, uint64_t host_surfels) {
   if (!c) return SB_ERR_INVALID;
   if (pool_surfels < kExtractCap || pool_surfels > kTilePoolCap)
     return fail(c, SB_ERR_INVALID, "set_tile_cache: pool_surfels must lie in [500000, 16777216]");
-  if (c->n_slots != 0 || !c->tiles.empty() || !c->tc.host.empty())
+  if (!c->pg.empty())
     return fail(c, SB_ERR_STATE, "set_tile_cache: the tile cache is not empty (call it after sb_create or sb_reset)");
-  c->tc.managed = true;
-  c->tc.pool_cap = pool_surfels;
-  c->tc.host_cap = host_surfels;
+  c->pg.setting = Paging::Setting{true, pool_surfels, host_surfels};
   return SB_OK;
 }
 
 int sb_get_tile_cache_info(sb_ctx* c, sb_tile_cache_info* o) {
   if (!c || !o) return SB_ERR_INVALID;
   cudaSetDevice(c->device);
-  std::vector<uint2> rec(c->n_slots);
-  if (c->n_slots) {  // read the records without changing what the context knows
-    SB_CUDA(c, cudaMemcpyAsync(rec.data(), c->d_tile_rec, rec.size() * sizeof(uint2), cudaMemcpyDeviceToHost, c->stream));
-    SB_CUDA(c, cudaStreamSynchronize(c->stream));
-  }
+  // read into a temporary: when the context reads the records back is observable (stats[12], the pool's error message)
+  TileRecords rec;
+  if (int r = read_tile_records(c, rec)) return r;
+  const Paging& pg = c->pg;
   memset(o, 0, sizeof(*o));
-  const sb_ctx::TileCache& tc = c->tc;
-  o->managed = tc.managed;
-  o->tiles_in_pool = (uint32_t)c->tiles.size();
-  o->tiles_on_host = (uint32_t)tc.host.size();
-  o->pool_capacity = tc.pool_cap;
-  o->pool_used = c->n_slots ? rec[c->n_slots - 1].x : 0u;
-  for (const auto& kv : c->tiles) {
-    const uint32_t s = kv.second.slot;
-    o->pool_referenced += rec[s].x - (s ? rec[s - 1].x : 0u);
-  }
-  o->host_capacity = tc.host_cap;
-  o->host_used = tc.host_used;
-  o->reclaims = tc.reclaims;
-  o->reclaim_moved = tc.reclaim_moved;
-  o->evictions = tc.evictions;
-  o->host_fills = tc.host_fills;
-  o->dropped = tc.dropped_retired;
-  for (uint32_t s = 0; s < c->n_slots; ++s) o->dropped += std::min(rec[s].y, kExtractCap) - (rec[s].x - (s ? rec[s - 1].x : 0u));
+  o->managed = pg.setting.managed;
+  o->tiles_in_pool = (uint32_t)pg.tiles.size();
+  o->tiles_on_host = (uint32_t)pg.host.size();
+  o->pool_capacity = pg.setting.pool_cap;
+  o->pool_used = rec.end();
+  for (const auto& kv : pg.tiles) o->pool_referenced += rec.size(kv.second);
+  o->host_capacity = pg.setting.host_cap;
+  o->host_used = pg.host_used;
+  o->reclaims = pg.counters.reclaims;
+  o->reclaim_moved = pg.counters.reclaim_moved;
+  o->evictions = pg.counters.evictions;
+  o->host_fills = pg.counters.host_fills;
+  o->dropped = pg.counters.dropped_retired + rec.dropped();
   return SB_OK;
 }
 
@@ -2437,6 +2432,100 @@ struct Reader {
 
 namespace lp = suma_b200::loop;
 
+// The paging state as a checkpoint holds it; a context derives `known`, base, count and `pending` from its record copy.
+struct PagingImage {
+  struct Tile { TileKey idx; uint32_t slot, known, base, count; };
+  // data: count surfels as four lanes of pitch count, in the pinned buffer (save) or in the blob (load)
+  struct HostTileImage { TileKey idx; uint32_t count; const uint8_t* data; };
+  int32_t origin_i = 0, origin_j = 0;
+  std::vector<TileKey> extraction;
+  std::vector<Tile> tiles;  // in index order
+  uint32_t n_slots = 0, pending = 0, pool_end = 0;
+  TileRecords rec;  // every slot's record, as on the device
+  // the managed cache (section S_TCACHE, written only by managed contexts)
+  Paging::Setting setting;
+  uint64_t pool_bound = 0, host_used = 0;
+  Paging::Counters counters;
+  std::vector<HostTileImage> host;  // in index order
+  uint32_t n_known() const {  // the lowest slot of an unknown tile
+    uint32_t n = n_slots;
+    for (const Tile& t : tiles) n = t.known ? n : std::min(n, t.slot);
+    return n;
+  }
+};
+
+// The context's paging state (the stream is synchronised: the evictions' copies have landed).
+int capture_paging(sb_ctx* c, PagingImage& g) {
+  const Paging& pg = c->pg;
+  g.origin_i = pg.origin_i; g.origin_j = pg.origin_j; g.extraction = pg.extraction;
+  g.tiles.clear();
+  for (const auto& kv : pg.tiles) {
+    const uint32_t s = kv.second, k = pg.known(s);
+    g.tiles.push_back({kv.first, s, k, k ? pg.rec.base(s) : 0u, k ? pg.rec.size(s) : 0u});
+  }
+  g.n_slots = pg.n_slots; g.pending = pg.pending();
+  if (int r = read_tile_records(c, g.rec)) return r;
+  g.pool_end = g.rec.end();
+  g.setting = pg.setting; g.pool_bound = pg.pool_bound; g.host_used = pg.host_used; g.counters = pg.counters;
+  g.host.clear();
+  for (const auto& kv : pg.host)
+    g.host.push_back({kv.first, kv.second.count, reinterpret_cast<const uint8_t*>(kv.second.buf.get())});
+  return SB_OK;
+}
+
+// The range checks of a checkpoint's paging state: nullptr when they hold, otherwise the reason.
+const char* check_paging(const PagingImage& g) {
+  if (g.n_slots > kMaxTileSlots || g.pool_end > kTilePoolCap || g.extraction.size() > kMaxTileSlots ||
+      g.tiles.size() > kMaxTileSlots)
+    return "checkpoint exceeds the map / tile-pool capacity";
+  if (g.rec.v.size() != g.n_slots || g.rec.end() != g.pool_end) return "malformed tile records";
+  // slot k holds [end of slot k - 1, rec[k].x), no more than the tile had surfels (or the extract cap allows)
+  for (uint32_t k = 0; k < g.n_slots; ++k)
+    if (g.rec.v[k].x < g.rec.base(k) || g.rec.size(k) > std::min(g.rec.v[k].y, kExtractCap))
+      return "malformed tile records";
+  // the tiles read back are those below every tile not read back, and each names exactly its slot's range
+  const uint32_t n_known = g.n_known();
+  for (const auto& t : g.tiles)
+    if (t.slot >= g.n_slots || (t.known && (t.slot >= n_known || t.base != g.rec.base(t.slot) ||
+                                            t.count != g.rec.size(t.slot))))
+      return "malformed tile table";
+  if ((g.pending != 0) != (n_known < g.n_slots)) return "malformed tile table";
+  if (!g.setting.managed) return nullptr;
+  // every count of the managed cache is checked against the saved capacities
+  if (g.setting.pool_cap < kExtractCap || g.setting.pool_cap > kTilePoolCap || g.pool_end > g.setting.pool_cap ||
+      g.pool_bound < g.pool_end)
+    return "malformed tile cache section (pool beyond its capacity)";
+  uint64_t host_total = 0;
+  for (const auto& t : g.host) host_total += t.count;
+  if (host_total != g.host_used || g.host_used > g.setting.host_cap)
+    return "malformed tile cache section (host tier beyond its capacity)";
+  for (size_t k = 0; k < g.host.size(); ++k) {  // strictly ordered by index, none also in the pool
+    if (k && !(g.host[k - 1].idx < g.host[k].idx)) return "malformed tile cache section (host tiles out of order)";
+    for (const auto& t : g.tiles)
+      if (t.idx == g.host[k].idx) return "malformed tile cache section (a tile in both tiers)";
+  }
+  return nullptr;
+}
+
+// Replaces the context's paging state and cache setting with a checked image (the caller uploads the device records).
+int apply_paging(sb_ctx* c, const PagingImage& g) {
+  Paging& pg = c->pg;
+  pg.clear();
+  pg.setting = g.setting;
+  pg.pool_bound = g.setting.managed ? g.pool_bound : g.pool_end;
+  pg.counters = g.counters;
+  for (const auto& t : g.host) {
+    HostTile* h;
+    if (int r = add_host_tile(c, t.idx, t.count, &h)) return r;
+    if (t.count) memcpy(h->buf.get(), t.data, (size_t)t.count * 64);
+  }
+  pg.origin_i = g.origin_i; pg.origin_j = g.origin_j; pg.extraction = g.extraction;
+  for (const auto& t : g.tiles) pg.tiles[t.idx] = t.slot;
+  pg.n_slots = g.n_slots;
+  pg.rec.v.assign(g.rec.v.begin(), g.rec.v.begin() + g.n_known());
+  return SB_OK;
+}
+
 // Everything a checkpoint holds except the three device-resident bulk sections (surfels, tile pool, frames).
 struct StateImage {
   sb_params p;
@@ -2446,24 +2535,10 @@ struct StateImage {
   double stats[16];
   uint32_t cur_has_semantics = 0, last_has_semantics = 0, close_loops = 0;
   uint32_t n_live = 0, map_timestamp = 0, pose_ref_end = 0, n_updated = 0, n_new = 0;
-  int32_t origin_i = 0, origin_j = 0;
-  std::vector<std::pair<int32_t, int32_t>> extraction;
-  std::vector<std::pair<std::pair<int32_t, int32_t>, DevTile>> tiles;
-  uint32_t n_slots = 0, tiles_pending = 0, pool_end = 0;
   std::vector<float> poses, poses_inv;  // the used entries of the device pose tables
   ResultBlock result;
-  std::vector<uint2> tile_rec;
   lp::State loop;
-  // the managed tile cache (section S_TCACHE, written only by managed contexts)
-  struct HostTileImage {
-    int32_t i, j;
-    uint32_t count;
-    const uint8_t* data;  // count surfels as four lanes of pitch count: the pinned buffer (save) or the blob (load)
-  };
-  uint32_t tc_managed = 0, tc_pool_cap = kTilePoolCap;
-  uint64_t tc_host_cap = 0, tc_pool_bound = 0, tc_host_used = 0, tc_reclaims = 0, tc_moved = 0, tc_evictions = 0,
-           tc_fills = 0, tc_dropped = 0;
-  std::vector<HostTileImage> host_tiles;
+  PagingImage paging;
   // the deskewing setting (section S_DESKEW, written only when deskewing is on)
   sb_deskew_params deskew{0, 0.5f, 3.14159265358979323846f, 1};
 };
@@ -2527,15 +2602,16 @@ void write_host_sections(Writer& w, const StateImage& s) {
   w.bytes(s.stats, sizeof(s.stats));
   w.put(s.trackLoss); w.put(s.cur_has_semantics); w.put(s.last_has_semantics); w.put(s.close_loops);
   w.put(s.n_live); w.put(s.map_timestamp); w.put(s.pose_ref_end); w.put(s.n_updated); w.put(s.n_new);
-  w.put(s.origin_i); w.put(s.origin_j);
-  w.put((uint32_t)s.extraction.size());
-  for (const auto& e : s.extraction) { w.put(e.first); w.put(e.second); }
-  w.put((uint32_t)s.tiles.size());
-  for (const auto& t : s.tiles) {
-    w.put(t.first.first); w.put(t.first.second);
-    w.put(t.second.slot); w.put((uint32_t)t.second.known); w.put(t.second.base); w.put(t.second.count);
+  const PagingImage& g = s.paging;
+  w.put(g.origin_i); w.put(g.origin_j);
+  w.put((uint32_t)g.extraction.size());
+  for (const auto& e : g.extraction) { w.put(e.first); w.put(e.second); }
+  w.put((uint32_t)g.tiles.size());
+  for (const auto& t : g.tiles) {
+    w.put(t.idx.first); w.put(t.idx.second);
+    w.put(t.slot); w.put(t.known); w.put(t.base); w.put(t.count);
   }
-  w.put(s.n_slots); w.put(s.tiles_pending); w.put(s.pool_end);
+  w.put(g.n_slots); w.put(g.pending); w.put(g.pool_end);
   w.close(o);
 
   o = w.open(S_LOOP);
@@ -2567,18 +2643,19 @@ void write_host_sections(Writer& w, const StateImage& s) {
   w.close(o);
 
   o = w.open(S_TILES);
-  w.put((uint32_t)s.tile_rec.size());
-  for (const uint2& r : s.tile_rec) { w.put(r.x); w.put(r.y); }
+  w.put((uint32_t)g.rec.v.size());
+  for (const uint2& r : g.rec.v) { w.put(r.x); w.put(r.y); }
   w.close(o);
 
-  if (!s.tc_managed) return write_deskew_section(w, s);  // a default context's checkpoint has no such section
+  if (!g.setting.managed) return write_deskew_section(w, s);  // a default context's checkpoint has no such section
   o = w.open(S_TCACHE);
-  w.put(s.tc_pool_cap); w.put((uint32_t)s.host_tiles.size());
-  for (uint64_t v : {s.tc_host_cap, s.tc_pool_bound, s.tc_host_used, s.tc_reclaims, s.tc_moved, s.tc_evictions, s.tc_fills,
-                     s.tc_dropped})
+  const Paging::Counters& n = g.counters;
+  w.put(g.setting.pool_cap); w.put((uint32_t)g.host.size());
+  for (uint64_t v : {g.setting.host_cap, g.pool_bound, g.host_used, n.reclaims, n.reclaim_moved, n.evictions,
+                     n.host_fills, n.dropped_retired})
     w.put(v);
-  for (const auto& t : s.host_tiles) { w.put(t.i); w.put(t.j); w.put(t.count); w.put(uint32_t(0)); }
-  for (const auto& t : s.host_tiles) w.bytes(t.data, (size_t)t.count * 64);
+  for (const auto& t : g.host) { w.put(t.idx.first); w.put(t.idx.second); w.put(t.count); w.put(uint32_t(0)); }
+  for (const auto& t : g.host) w.bytes(t.data, (size_t)t.count * 64);
   w.close(o);
   write_deskew_section(w, s);
 }
@@ -2602,8 +2679,6 @@ uint32_t peek_section(const Reader& r) {
   if (r.ok && r.n - r.off >= 4) memcpy(&next, r.p + r.off, 4);
   return next;
 }
-const char* read_tile_cache(Reader& r, StateImage& s);
-
 // Parses the header and the host sections; nullptr when they are well formed, otherwise the reason.
 const char* read_host(Reader& r, const sb_ctx* c, StateImage& s) {
   char magic[8];
@@ -2646,24 +2721,21 @@ const char* read_host(Reader& r, const sb_ctx* c, StateImage& s) {
   s.close_loops = r.get<uint32_t>();
   s.n_live = r.get<uint32_t>(); s.map_timestamp = r.get<uint32_t>(); s.pose_ref_end = r.get<uint32_t>();
   s.n_updated = r.get<uint32_t>(); s.n_new = r.get<uint32_t>();
-  s.origin_i = r.get<int32_t>(); s.origin_j = r.get<int32_t>();
-  s.extraction.resize(r.count(8));
-  for (auto& e : s.extraction) { e.first = r.get<int32_t>(); e.second = r.get<int32_t>(); }
-  s.tiles.resize(r.count(24));
-  for (auto& t : s.tiles) {
-    t.first.first = r.get<int32_t>(); t.first.second = r.get<int32_t>();
-    t.second.slot = r.get<uint32_t>(); t.second.known = r.get<uint32_t>() != 0;
-    t.second.base = r.get<uint32_t>(); t.second.count = r.get<uint32_t>();
+  PagingImage& g = s.paging;
+  g.origin_i = r.get<int32_t>(); g.origin_j = r.get<int32_t>();
+  g.extraction.resize(r.count(8));
+  for (auto& e : g.extraction) { e.first = r.get<int32_t>(); e.second = r.get<int32_t>(); }
+  g.tiles.resize(r.count(24));
+  for (auto& t : g.tiles) {
+    t.idx.first = r.get<int32_t>(); t.idx.second = r.get<int32_t>();
+    t.slot = r.get<uint32_t>(); t.known = r.get<uint32_t>() != 0;
+    t.base = r.get<uint32_t>(); t.count = r.get<uint32_t>();
   }
-  s.n_slots = r.get<uint32_t>(); s.tiles_pending = r.get<uint32_t>(); s.pool_end = r.get<uint32_t>();
+  g.n_slots = r.get<uint32_t>(); g.pending = r.get<uint32_t>(); g.pool_end = r.get<uint32_t>();
   if (!read_close(r, start, len)) return "malformed state section";
   // A digest is no signature: every field that later sizes a copy or indexes device memory is range-checked here.
-  if (s.n_live > kMaxSurfels || s.n_slots > kMaxTileSlots || s.pool_end > kTilePoolCap ||
-      s.extraction.size() > kMaxTileSlots || s.tiles.size() > kMaxTileSlots)
-    return "checkpoint exceeds the map / tile-pool capacity";
+  if (s.n_live > kMaxSurfels) return "checkpoint exceeds the map / tile-pool capacity";
   if (s.pose_ref_end > kMaxPoses) return "malformed map state (pose-table reference beyond the table)";
-  for (const auto& t : s.tiles)
-    if (t.second.slot >= s.n_slots) return "malformed tile table";
 
   len = read_open(r, S_LOOP);
   start = r.off;
@@ -2716,24 +2788,34 @@ const char* read_host(Reader& r, const sb_ctx* c, StateImage& s) {
 
   len = read_open(r, S_TILES);
   start = r.off;
-  s.tile_rec.resize(r.count(8));
-  for (uint2& t : s.tile_rec) { t.x = r.get<uint32_t>(); t.y = r.get<uint32_t>(); }
-  if (!read_close(r, start, len) || s.tile_rec.size() != s.n_slots) return "malformed tile records";
-  if ((s.n_slots ? s.tile_rec[s.n_slots - 1].x : 0u) != s.pool_end) return "malformed tile records";
-  // slot k holds [end of slot k - 1, rec[k].x), no more than the tile had surfels (or the extract cap allows)
-  for (uint32_t k = 0; k < s.n_slots; ++k) {
-    const uint32_t base = k ? s.tile_rec[k - 1].x : 0u;
-    if (s.tile_rec[k].x < base || s.tile_rec[k].x - base > std::min(s.tile_rec[k].y, kExtractCap))
-      return "malformed tile records";
-  }
-  for (const auto& t : s.tiles) {  // a tile already read back names exactly its slot's range
-    const uint32_t base = t.second.slot ? s.tile_rec[t.second.slot - 1].x : 0u;
-    if (t.second.known && (t.second.base != base || t.second.count != s.tile_rec[t.second.slot].x - base))
-      return "malformed tile table";
-  }
+  g.rec.v.resize(r.count(8));
+  for (uint2& t : g.rec.v) { t.x = r.get<uint32_t>(); t.y = r.get<uint32_t>(); }
+  if (!read_close(r, start, len)) return "malformed tile records";
 
-  if (peek_section(r) == S_TCACHE)
-    if (const char* why = read_tile_cache(r, s)) return why;
+  if (peek_section(r) == S_TCACHE) {  // the managed cache: the setting, the counters and the host tiles
+    len = read_open(r, S_TCACHE);
+    start = r.off;
+    Paging::Counters& n = g.counters;
+    g.setting.managed = true;
+    g.setting.pool_cap = r.get<uint32_t>();
+    g.host.resize(r.count(16));
+    for (uint64_t* v : {&g.setting.host_cap, &g.pool_bound, &g.host_used, &n.reclaims, &n.reclaim_moved, &n.evictions,
+                        &n.host_fills, &n.dropped_retired})
+      *v = r.get<uint64_t>();
+    uint64_t host_total = 0;
+    for (auto& t : g.host) {
+      t.idx.first = r.get<int32_t>(); t.idx.second = r.get<int32_t>(); t.count = r.get<uint32_t>(); r.get<uint32_t>();
+      if (t.count > kExtractCap) return "malformed tile cache section (host tile over the extract cap)";
+      host_total += t.count;
+    }
+    if (!r.ok || host_total * 64 > r.n - r.off) return "malformed tile cache section";
+    for (auto& t : g.host) {
+      t.data = r.p + r.off;
+      r.off += (size_t)t.count * 64;
+    }
+    if (!read_close(r, start, len)) return "malformed tile cache section";
+  }
+  if (const char* why = check_paging(g)) return why;
   if (peek_section(r) != S_DESKEW) return nullptr;  // a checkpoint without the section loads with deskewing off
   len = read_open(r, S_DESKEW);
   start = r.off;
@@ -2744,44 +2826,6 @@ const char* read_host(Reader& r, const sb_ctx* c, StateImage& s) {
   if (!read_close(r, start, len)) return "malformed deskew section";
   if (check_deskew(&s.deskew) || s.deskew.mode == 0 || (s.deskew.clockwise != 0 && s.deskew.clockwise != 1))
     return "malformed deskew section (setting out of range)";
-  return nullptr;
-}
-
-// The managed tile cache's section: the setting, the counters and the host tiles, range-checked.
-const char* read_tile_cache(Reader& r, StateImage& s) {
-  uint64_t len = read_open(r, S_TCACHE);
-  const size_t start = r.off;
-  s.tc_managed = 1;
-  s.tc_pool_cap = r.get<uint32_t>();
-  s.host_tiles.resize(r.count(16));
-  for (uint64_t* v : {&s.tc_host_cap, &s.tc_pool_bound, &s.tc_host_used, &s.tc_reclaims, &s.tc_moved, &s.tc_evictions,
-                      &s.tc_fills, &s.tc_dropped})
-    *v = r.get<uint64_t>();
-  uint64_t host_total = 0;
-  for (auto& t : s.host_tiles) {
-    t.i = r.get<int32_t>(); t.j = r.get<int32_t>(); t.count = r.get<uint32_t>(); r.get<uint32_t>();
-    if (t.count > kExtractCap) return "malformed tile cache section (host tile over the extract cap)";
-    host_total += t.count;
-  }
-  if (!r.ok || host_total * 64 > r.n - r.off) return "malformed tile cache section";
-  for (auto& t : s.host_tiles) {
-    t.data = r.p + r.off;
-    r.off += (size_t)t.count * 64;
-  }
-  if (!read_close(r, start, len)) return "malformed tile cache section";
-  // every count is checked against the saved capacities before anything changes
-  if (s.tc_pool_cap < kExtractCap || s.tc_pool_cap > kTilePoolCap || s.pool_end > s.tc_pool_cap ||
-      s.tc_pool_bound < s.pool_end)
-    return "malformed tile cache section (pool beyond its capacity)";
-  if (host_total != s.tc_host_used || s.tc_host_used > s.tc_host_cap)
-    return "malformed tile cache section (host tier beyond its capacity)";
-  for (size_t k = 0; k < s.host_tiles.size(); ++k) {  // strictly ordered by index, none also in the pool
-    const auto key = std::make_pair(s.host_tiles[k].i, s.host_tiles[k].j);
-    if (k && !(std::make_pair(s.host_tiles[k - 1].i, s.host_tiles[k - 1].j) < key))
-      return "malformed tile cache section (host tiles out of order)";
-    for (const auto& t : s.tiles)
-      if (t.first == key) return "malformed tile cache section (a tile in both tiers)";
-  }
   return nullptr;
 }
 
@@ -2810,7 +2854,7 @@ std::vector<DevSection> dev_sections(sb_ctx* c, uint32_t n_live, uint32_t pool_e
   d[0].id = S_SURFELS;
   d[0].ranges.push_back(DevRange{c->T.p0, (uint64_t)n_live * 64});
   d[1].id = S_POOL;
-  for (float4* lane : {c->pool.p0, c->pool.p1, c->pool.p2, c->pool.p3})
+  for (float4* lane : {c->pg.pool.p0, c->pg.pool.p1, c->pg.pool.p2, c->pg.pool.p3})
     d[1].ranges.push_back(DevRange{lane, (uint64_t)pool_end * 16});
   d[2].id = S_FRAMES;
   const sb_frame* f[7];
@@ -2923,24 +2967,7 @@ int capture(sb_ctx* c, StateImage& s) {
   s.n_live = n_live(c);
   s.map_timestamp = c->map_timestamp; s.pose_ref_end = c->pose_ref_end;
   s.n_updated = c->n_updated; s.n_new = c->n_new;
-  s.origin_i = c->origin_i; s.origin_j = c->origin_j;
-  s.extraction = c->extraction;
-  s.tiles.assign(c->tiles.begin(), c->tiles.end());
-  s.n_slots = c->n_slots;
-  s.tiles_pending = c->tiles_pending;
-  s.tile_rec.resize(c->n_slots);
-  if (c->n_slots)
-    SB_CUDA(c, cudaMemcpy(s.tile_rec.data(), c->d_tile_rec, (size_t)c->n_slots * sizeof(uint2), cudaMemcpyDeviceToHost));
-  s.pool_end = c->n_slots ? s.tile_rec[c->n_slots - 1].x : 0u;
-  const sb_ctx::TileCache& tc = c->tc;
-  s.tc_managed = tc.managed;
-  s.tc_pool_cap = tc.pool_cap;
-  s.tc_host_cap = tc.host_cap; s.tc_pool_bound = tc.pool_bound; s.tc_host_used = tc.host_used;
-  s.tc_reclaims = tc.reclaims; s.tc_moved = tc.reclaim_moved; s.tc_evictions = tc.evictions; s.tc_fills = tc.host_fills; s.tc_dropped = tc.dropped_retired;
-  s.host_tiles.clear();
-  for (const auto& kv : tc.host)  // (the stream is synchronised: the evictions' copies have landed)
-    s.host_tiles.push_back(StateImage::HostTileImage{kv.first.first, kv.first.second, kv.second.count,
-                                                     reinterpret_cast<const uint8_t*>(kv.second.buf.get())});
+  if (int r = capture_paging(c, s.paging)) return r;
   // the used entries of the pose tables: those the map can refer to, and any set beyond them through sb_map_set_pose
   uint32_t np = pose_table_count(c);
   for (uint32_t t = kMaxPoses; t > np; --t) {
@@ -2961,33 +2988,9 @@ int capture(sb_ctx* c, StateImage& s) {
   return SB_OK;
 }
 
-// The host tier of a checkpoint replaces the context's (and with it the cache setting).
-int apply_tile_cache(sb_ctx* c, const StateImage& s) {
-  sb_ctx::TileCache& tc = c->tc;
-  for (auto& kv : tc.host) release_host_tile(c, kv.second);
-  tc.host.clear();
-  tc.host_used = 0;
-  tc.managed = s.tc_managed != 0;
-  tc.pool_cap = s.tc_managed ? s.tc_pool_cap : kTilePoolCap;
-  tc.host_cap = s.tc_host_cap;
-  tc.pool_bound = s.tc_managed ? s.tc_pool_bound : s.pool_end;
-  tc.reclaims = s.tc_reclaims; tc.reclaim_moved = s.tc_moved; tc.evictions = s.tc_evictions; tc.host_fills = s.tc_fills;
-  tc.dropped_retired = s.tc_dropped;
-  for (const auto& t : s.host_tiles) {
-    HostTile h;
-    h.count = t.count;
-    int r;
-    if ((r = acquire_host_buffer(c, h))) return r;
-    if (t.count) memcpy(h.buf.get(), t.data, (size_t)t.count * 64);
-    tc.host_used += t.count;
-    tc.host[std::make_pair(t.i, t.j)] = std::move(h);
-  }
-  return SB_OK;
-}
-
 // Commits a verified checkpoint (the bulk sections are already on the device).
 int apply(sb_ctx* c, const StateImage& s) {
-  if (int r = apply_tile_cache(c, s)) {
+  if (int r = apply_paging(c, s.paging)) {
     const std::string why = c->err;
     reset_state(c);  // never leave a half-loaded context behind
     return fail(c, r, why + "; the context was reset");
@@ -3010,12 +3013,6 @@ int apply(sb_ctx* c, const StateImage& s) {
   c->prepped_for_update = false;
   c->map_timestamp = s.map_timestamp; c->pose_ref_end = s.pose_ref_end;
   c->n_updated = s.n_updated; c->n_new = s.n_new;
-  c->origin_i = s.origin_i; c->origin_j = s.origin_j;
-  c->extraction = s.extraction;
-  c->tiles.clear();
-  for (const auto& t : s.tiles) c->tiles[t.first] = t.second;
-  c->n_slots = s.n_slots;
-  c->tiles_pending = s.tiles_pending != 0;
   c->h_poses.assign((size_t)kMaxPoses * 16, 0.0f);
   for (uint32_t t = 0; t < kMaxPoses; ++t)
     for (int i = 0; i < 4; ++i) c->h_poses[16 * (size_t)t + 5 * i] = 1.0f;
@@ -3027,9 +3024,9 @@ int apply(sb_ctx* c, const StateImage& s) {
                              c->stream));
   c->host->result = s.result;
   SB_CUDA(c, cudaMemcpyAsync(c->res, &c->host->result, sizeof(ResultBlock), cudaMemcpyHostToDevice, c->stream));
-  if (s.n_slots)
-    SB_CUDA(c, cudaMemcpyAsync(c->d_tile_rec, s.tile_rec.data(), (size_t)s.n_slots * sizeof(uint2), cudaMemcpyHostToDevice,
-                               c->stream));
+  const std::vector<uint2>& rec = s.paging.rec.v;
+  if (!rec.empty())
+    SB_CUDA(c, cudaMemcpyAsync(c->pg.d_rec, rec.data(), rec.size() * sizeof(uint2), cudaMemcpyHostToDevice, c->stream));
   // scratch that a scan expects as the previous one left it: key images cleared by the pass that consumed them, group
   // totals zero (a context that stopped mid-scan may not hold these; a loaded one does)
   const size_t Pm = (size_t)c->kp.Wm * c->kp.Hm, Pk = preprocess_key_elems(c->kp.W, c->kp.H);
@@ -3047,7 +3044,7 @@ void layout(sb_ctx* c, const StateImage& s, Writer& head, std::vector<DevSection
             uint64_t* total) {
   Writer w;
   write_host_sections(w, s);
-  dev = dev_sections(c, s.n_live, s.pool_end);
+  dev = dev_sections(c, s.n_live, s.paging.pool_end);
   Writer hdr;
   write_header(hdr, s, 0);
   uint64_t off = hdr.b.size() + w.b.size();
@@ -3136,7 +3133,7 @@ int sb_state_load(sb_ctx* c, const void* src, uint64_t n) {
   Reader rd{static_cast<const uint8_t*>(src), (size_t)n};
   if (const char* why = read_host(rd, c, s)) return fail(c, SB_ERR_INVALID, std::string("state_load: ") + why);
   cudaSetDevice(c->device);
-  std::vector<DevSection> dev = dev_sections(c, s.n_live, s.pool_end);
+  std::vector<DevSection> dev = dev_sections(c, s.n_live, s.paging.pool_end);
   uint64_t off[3];
   for (int i = 0; i < 3; ++i) {
     const uint64_t len = read_open(rd, dev[i].id);

@@ -290,6 +290,14 @@ def _section(blob, sid):
         off += 16 + n
 
 
+def _tile_table(blob):
+    """offset and rows (i, j, slot, known, base, count) of the tile table in section S_HOST, offset of tiles_pending"""
+    n_ext = int(np.frombuffer(blob, np.uint32, 1, _section(blob, 1) + 952)[0])
+    at = _section(blob, 1) + 956 + 8 * n_ext
+    n = int(np.frombuffer(blob, np.uint32, 1, at)[0])
+    return at + 4, np.frombuffer(blob, np.uint32, 6 * n, at + 4).reshape(-1, 6), at + 4 + 24 * n + 4
+
+
 def _rc_load(g, blob):
     a = np.frombuffer(blob, np.uint8)
     rc = api.lib().sb_state_load(g.ctx.h, api._vp(a) if a.size else None, a.size)
@@ -335,6 +343,30 @@ def test_bad_checkpoints_are_refused():
     for t in range(3, 6):
         g.processScan(*sc[t])
         same(observe(g), obs[t + 1], "after refused loads t=%d" % t)
+    # tile tables whose records read back are not those of the lowest slots, or whose pending flag disagrees with them
+    _, ppp = both_params(**sized(128, 16))
+    paged = _Paged(ppp)
+    try:
+        paged.m.upload(np.concatenate([tile_surfels(3000, -4, k, 10 + k) for k in range(-4, 5)]), 1)
+        for x in (12, 12):  # two tiles of column -4 extracted (partial extraction), neither read back
+            paged.m.update(pose_at(x), paged.f)
+        pblob = paged.g.save_state()
+        before = observe(paged.g)
+        at, tiles, pending_at = _tile_table(pblob)
+        assert (tiles[:, 3] == 0).all() and len(tiles) == 2 and np.frombuffer(pblob, np.uint32, 1, pending_at)[0] == 1
+        rec = np.frombuffer(pblob, np.uint32, 2 * 2, _section(pblob, 5) + 4).reshape(-1, 2)
+        k = int(np.argmax(tiles[:, 2]))  # the later extraction marked as read back, with its slot's exact range
+        base = int(rec[tiles[k, 2] - 1, 0]) if tiles[k, 2] else 0
+        not_prefix = bytearray(pblob)
+        not_prefix[at + 24 * k + 12:at + 24 * k + 24] = np.array([1, base, rec[tiles[k, 2], 0] - base], np.uint32).tobytes()
+        not_pending = bytearray(pblob)
+        not_pending[pending_at:pending_at + 4] = np.uint32(0).tobytes()
+        for what, b in [("a tile read back above one that is not", not_prefix), ("pending flag cleared", not_pending)]:
+            rc, msg = _rc_load(paged.g, bytes(b))
+            assert rc == -1 and "malformed tile table" in msg, "%s: %d %r" % (what, rc, msg)
+        same(observe(paged.g), before, "after refused tile tables")
+    finally:
+        paged.close()
     # multi-GPU exchange set up: both calls refuse
     cb = C.CFUNCTYPE(C.c_int, C.c_void_p, C.POINTER(C.c_int64))(lambda u, s: 0)
     assert api.lib().sb_comm_set_callback(g.ctx.h, C.cast(cb, C.c_void_p), None, 0, 64) == 0
