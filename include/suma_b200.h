@@ -156,13 +156,27 @@ int sb_ldlt_solve6(const double A[36], const double b[6], double x[6]);
 int sb_gn_step(const double out48[48], double last_error, double eps, double delta, double pose[16], double dx[6]);
 
 /* ---- K6: SurfelMap::update, SurfelMap.cpp:492-584 (+ paging :708-824) ------------------------------------------ */
+/* ---- pose table (DESIGN.md section 12). Each surfel refers to the pose-table entry of the scan that created it. The
+ * table starts at the reference's 10 000 entries (SurfelMap.h:205) and doubles, at a call boundary, before any entry at
+ * or beyond it is written or referenced: by sb_process_scan / sb_process_scan_timed / sb_map_update (entry
+ * sb_map_timestamp), sb_map_set_pose (entry t), sb_map_update_poses / sb_integrate_loop_closures (entries [0, count)),
+ * sb_map_upload (the largest entry its surfels refer to) and sb_state_load (the checkpoint's size). The last entry is
+ * 16 777 215 (2^24 - 1: the float count field holds larger integers inexactly); a call that needs more returns
+ * SB_ERR_CAPACITY, and one whose allocation fails SB_ERR_NOMEM, both before anything changes. sb_reset returns to 10 000.
+ * The per-scan product tables inv(P) * poses[t] cover only the entries the active map can refer to: none of this changes
+ * a result bit. */
 int sb_map_update(sb_ctx* ctx, const float pose[16], const sb_frame* frame);
 int sb_map_update_poses(sb_ctx* ctx, const float* poses16, uint32_t count); /* SurfelMap::updatePoses :485 */
 int sb_map_size(sb_ctx* ctx, uint32_t* n);                                  /* SurfelMap::size */
 int sb_map_timestamp(sb_ctx* ctx, uint32_t* t);
 int sb_map_download(sb_ctx* ctx, sb_surfel* dst, uint32_t cap, uint32_t* n); /* SurfelMap::getAllSurfels */
-int sb_map_upload(sb_ctx* ctx, const sb_surfel* src, uint32_t n, uint32_t timestamp); /* test / restore hook */
-int sb_map_set_pose(sb_ctx* ctx, uint32_t t, const float pose[16]);
+/* test / restore hook: replaces the active map and sets its timestamp; SB_ERR_CAPACITY for a surfel whose count is
+   2^24 or more */
+int sb_map_upload(sb_ctx* ctx, const sb_surfel* src, uint32_t n, uint32_t timestamp);
+int sb_map_set_pose(sb_ctx* ctx, uint32_t t, const float pose[16]); /* any t < 2^24: the table grows to hold it */
+/* the pose table's size (capacity) and the window [begin, end) over which the product tables are computed: begin is a
+   lower bound on the smallest entry a live surfel of the active map refers to (any pointer may be NULL) */
+int sb_pose_table_info(sb_ctx* ctx, uint32_t* capacity, uint32_t* begin, uint32_t* end);
 /* intermediates of the last update (any pointer may be NULL): index map (id+1), radius map, integrated flags.
    After sb_map_update the ids index the surfels in order (as sb_map_download returns them); after sb_process_scan they
    are the map's physical slots, which may include slots of surfels removed by in-place updates (same relative order). */
@@ -297,7 +311,10 @@ int sb_get_statistics(sb_ctx* ctx, double stats[16]);
  *    its digest has dropped them with the rest of the context's state.
  *  - both return SB_ERR_STATE while a multi-GPU exchange is set up.
  *  - a map with surfels removed in place is restored dense: only the physical slot ids that sb_map_update_debug reports
- *    after the next sb_process_scan can differ. */
+ *    after the next sb_process_scan can differ
+ *  - the header's pose capacity is the context's pose-table size (10 000 unless the table grew). A load accepts sizes
+ *    from 10 000 to 2^24 and gives the loading context the checkpoint's size (SB_ERR_NOMEM, nothing changed, when that
+ *    allocation fails); libraries without a growing table refuse a checkpoint of a grown one. */
 int sb_state_size(sb_ctx* ctx, uint64_t* bytes);
 int sb_state_save(sb_ctx* ctx, void* dst, uint64_t cap, uint64_t* written);
 int sb_state_load(sb_ctx* ctx, const void* src, uint64_t n);

@@ -155,6 +155,7 @@ def lib(build_if_missing=True):
         "sb_gn_step": [pd, f64, f64, f64, pd, pd],
         "sb_ldlt_solve6": [pd, pd, pd],
         "sb_map_update": [vp, pf, vp], "sb_map_update_poses": [vp, pf, u32], "sb_map_set_pose": [vp, u32, pf],
+        "sb_pose_table_info": [vp, C.POINTER(u32), C.POINTER(u32), C.POINTER(u32)],
         "sb_map_size": [vp, C.POINTER(u32)], "sb_map_timestamp": [vp, C.POINTER(u32)],
         "sb_map_download": [vp, vp, u32, C.POINTER(u32)], "sb_map_upload": [vp, vp, u32, u32],
         "sb_map_update_debug": [vp, vp, vp, vp, C.POINTER(u32), C.POINTER(u32)],
@@ -202,7 +203,7 @@ EXPORTED_SYMBOLS = [
     "sb_map_render_inactive", "sb_map_render_composed", "sb_map_frame", "sb_icp_jacobian", "sb_icp_unpack",
     "sb_icp_minimize", "sb_se3_exp", "sb_se3_log", "sb_ldlt_solve6", "sb_gn_step", "sb_map_update",
     "sb_map_update_poses", "sb_map_size", "sb_map_timestamp", "sb_map_download", "sb_map_upload", "sb_map_set_pose",
-    "sb_map_update_debug", "sb_map_submap_origin", "sb_process_scan", "sb_prefetch_scan", "sb_get_pose", "sb_get_last_pose", "sb_timestamp", "sb_slam_frame",
+    "sb_map_update_debug", "sb_map_submap_origin", "sb_pose_table_info", "sb_process_scan", "sb_prefetch_scan", "sb_get_pose", "sb_get_last_pose", "sb_timestamp", "sb_slam_frame",
     "sb_get_statistics", "sb_comm_export", "sb_comm_init", "sb_comm_shutdown", "sb_comm_set_callback",
     "sb_profile_enable", "sb_default_loop_params", "sb_set_loop_closure", "sb_get_loop_info", "sb_get_loop_edges",
     "sb_set_current_pose", "sb_integrate_loop_closures",
@@ -311,6 +312,12 @@ class Context:
         o = TileCacheInfo()
         self.check(lib().sb_get_tile_cache_info(self.h, C.byref(o)), "get_tile_cache_info")
         return {n: int(getattr(o, n)) for n, _ in TileCacheInfo._fields_ if n != "pad"}
+
+    def pose_table_info(self):
+        """the pose table's capacity and the window [begin, end) of its product tables (sb_pose_table_info) as a dict"""
+        cap, b, e = C.c_uint32(), C.c_uint32(), C.c_uint32()
+        self.check(lib().sb_pose_table_info(self.h, C.byref(cap), C.byref(b), C.byref(e)), "pose_table_info")
+        return {"capacity": cap.value, "begin": b.value, "end": e.value}
 
     def set_params(self, params):
         self.check(lib().sb_set_params(self.h, C.byref(params)), "set_params")
@@ -608,6 +615,9 @@ class SurfelMap:
     def tile_cache_info(self):
         return self.ctx.tile_cache_info()
 
+    def pose_table_info(self):
+        return self.ctx.pose_table_info()
+
     def reset(self):
         self.ctx.check(lib().sb_reset(self.ctx.h), "reset")
 
@@ -741,6 +751,9 @@ class SurfelMapping:
 
     def tile_cache_info(self):
         return self.ctx.tile_cache_info()
+
+    def pose_table_info(self):
+        return self.ctx.pose_table_info()
 
     def getStatistics(self):
         a = np.zeros(16)

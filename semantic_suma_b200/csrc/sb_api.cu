@@ -162,7 +162,7 @@ struct sb_ctx {
   DevPtr<uint32_t> lb_ticket;
   uint32_t lb_gen = 0;
   DevPtr<ResultBlock> res;  // pose block, statistics sums and surfel counts of the scan
-  DevPtr<float> poses;      // device pose table, kMaxPoses x 16
+  DevPtr<float> poses;      // device pose table, pose_cap x 16
   DevPtr<float> poses_inv;
   std::vector<float> h_poses, h_poses_inv;
   DevPtr<float> Mtab_old;
@@ -185,6 +185,15 @@ struct sb_ctx {
   // one past the largest pose-table entry a surfel of the map or of a cached tile can refer to (creation timestamp,
   // clamped as pose_index() does): while it is <= map_timestamp, no surfel reads the entry the scan's pose goes into
   uint32_t pose_ref_end = 0;
+  // Entries of the pose tables (poses, poses_inv, Mtab_old, Mtab_new and the host mirrors): kPoseCapInit, doubled at a call
+  // boundary before any entry at or beyond it is written or referenced (reserve_poses; DESIGN.md section 12).
+  uint32_t pose_cap = kPoseCapInit;
+  // A lower bound on the smallest entry a live surfel of the map refers to: the product tables inv(P) * poses[t] are
+  // computed over [pose_ref_begin, pose_window_end()) only. The extraction passes lower counts[8] to the smallest entry they
+  // see; the host absorbs it with the results of the next scan (pose_min_pending) unless the map gained older surfels since.
+  uint32_t pose_ref_begin = 0;
+  bool pose_min_pending = false;
+  uint32_t pose_min_floor = 0;  // map timestamp at the first pending pass: surfels created later refer to entries >= it
   Paging pg;
 
   // Full-render memo: SurfelMapping re-renders the unchanged map at the unchanged pose at the start of the next scan
@@ -301,6 +310,7 @@ void derive(sb_ctx* c) {
   k.map_max_distance = p.map_max_distance;
   k.max_loop_closure_distance = p.max_loop_closure_distance;
   k.label_offset_quirk = p.label_offset_quirk;
+  k.pose_cap = c->pose_cap;
   c->confidence_threshold = p.confidence_threshold;  // SurfelMapping.cpp:111-113
   float pu = 0.1f;
   c->log_unstable_slam = logf(pu / (1.0f - pu));     // SurfelMapping.cpp:108-109
@@ -354,21 +364,91 @@ int add_host_tile(sb_ctx* c, const TileKey& idx, uint32_t count, HostTile** out)
   return SB_OK;
 }
 
+// (Re)allocates the pose tables and their host mirrors at `cap` entries: entries [0, keep) of poses / poses_inv keep their
+// values, the others are identity (SurfelMap.cpp:473-482); Mtab_old / Mtab_new hold nothing until the next product pass.
+// Nothing changes when an allocation fails.
+int resize_pose_tables(sb_ctx* c, uint32_t cap, uint32_t keep) {
+  const size_t bytes = (size_t)cap * 64;
+  DevPtr<float> np, ni, mo, mn;
+  if (dev_alloc(np, bytes) != cudaSuccess || dev_alloc(ni, bytes) != cudaSuccess || dev_alloc(mo, bytes) != cudaSuccess ||
+      dev_alloc(mn, bytes) != cudaSuccess) {
+    cudaGetLastError();
+    return fail(c, SB_ERR_NOMEM, "pose table: out of device memory for " + std::to_string(cap) + " entries");
+  }
+  std::vector<float> hp, hi;
+  try {
+    hp.assign((size_t)cap * 16, 0.0f);
+    for (uint32_t t = keep; t < cap; ++t)
+      for (int i = 0; i < 4; ++i) hp[16 * (size_t)t + 5 * i] = 1.0f;
+    hi = hp;
+  } catch (const std::bad_alloc&) {
+    return fail(c, SB_ERR_NOMEM, "pose table: out of host memory for " + std::to_string(cap) + " entries");
+  }
+  memcpy(hp.data(), c->h_poses.data(), (size_t)keep * 64);
+  memcpy(hi.data(), c->h_poses_inv.data(), (size_t)keep * 64);
+  if (keep) {
+    SB_CUDA(c, cudaMemcpyAsync(np, c->poses, (size_t)keep * 64, cudaMemcpyDeviceToDevice, c->stream));
+    SB_CUDA(c, cudaMemcpyAsync(ni, c->poses_inv, (size_t)keep * 64, cudaMemcpyDeviceToDevice, c->stream));
+  }
+  SB_CUDA(c, cudaMemcpyAsync(np + 16 * (size_t)keep, &hp[16 * (size_t)keep], (size_t)(cap - keep) * 64,
+                             cudaMemcpyHostToDevice, c->stream));
+  SB_CUDA(c, cudaMemcpyAsync(ni + 16 * (size_t)keep, &hp[16 * (size_t)keep], (size_t)(cap - keep) * 64,
+                             cudaMemcpyHostToDevice, c->stream));
+  SB_CUDA(c, cudaStreamSynchronize(c->stream));  // the copies read the old tables and the host vectors
+  c->poses = std::move(np); c->poses_inv = std::move(ni); c->Mtab_old = std::move(mo); c->Mtab_new = std::move(mn);
+  c->h_poses.swap(hp);
+  c->h_poses_inv.swap(hi);
+  c->pose_cap = cap;
+  c->kp.pose_cap = cap;
+  c->map_version += 1;
+  return SB_OK;
+}
+
+// Grows the pose tables (doubling) so that entries [0, need) exist. Refused past kPoseCapMax before anything changes.
+int reserve_poses(sb_ctx* c, uint64_t need) {
+  if (need <= c->pose_cap) return SB_OK;
+  if (need > kPoseCapMax)
+    return fail(c, SB_ERR_CAPACITY, "pose table: entry " + std::to_string(need - 1) +
+                                        " is beyond the last one, 16777215 (a surfel keeps its entry in a float)");
+  uint64_t cap = c->pose_cap;
+  while (cap < need) cap *= 2;
+  return resize_pose_tables(c, (uint32_t)std::min<uint64_t>(cap, kPoseCapMax), c->pose_cap);
+}
+
+// The map may hold surfels older than the bound (re-inserted tiles, restored state): back to 0 until the next extraction.
+void lower_pose_ref(sb_ctx* c, uint32_t begin = 0) {
+  c->pose_ref_begin = begin;
+  c->pose_min_pending = false;
+}
+
+// counts[8] as the results of a scan read it back: the extraction passes' minimum becomes the bound
+void absorb_pose_min(sb_ctx* c, uint32_t pose_min) {
+  if (!c->pose_min_pending) return;
+  c->pose_ref_begin = pose_min < c->pose_min_floor ? pose_min : c->pose_min_floor;
+  c->pose_min_pending = false;
+}
+
 int reset_state(sb_ctx* c) {
   // SurfelMap::reset (SurfelMap.cpp:473-482) + the SurfelMapping members set up in its constructor
   c->map_version += 1;
   c->n_host = 0; c->n_holes = 0; c->lazy_update = false;
   c->n_updated = 0; c->n_new = 0; c->map_timestamp = 0; c->pose_ref_end = 0;
+  lower_pose_ref(c);
   c->pg.clear();
   c->stats[12] = 0.0;
   c->loop.reset();  // posegraph_->clear(); trajectory_distances_ ... (SurfelMapping.cpp:158-163)
   for (int i = 0; i < 16; ++i) c->lastPose_old[i] = (i % 5 == 0) ? 1.0 : 0.0;
-  c->h_poses.assign((size_t)kMaxPoses * 16, 0.0f);
-  for (uint32_t t = 0; t < kMaxPoses; ++t)
-    for (int i = 0; i < 4; ++i) c->h_poses[16 * (size_t)t + 5 * i] = 1.0f;
-  c->h_poses_inv = c->h_poses;
-  SB_CUDA(c, cudaMemcpyAsync(c->poses, c->h_poses.data(), (size_t)kMaxPoses * 64, cudaMemcpyHostToDevice, c->stream));
-  SB_CUDA(c, cudaMemcpyAsync(c->poses_inv, c->h_poses.data(), (size_t)kMaxPoses * 64, cudaMemcpyHostToDevice, c->stream));
+  if (c->pose_cap != kPoseCapInit) {  // a grown table goes back to the initial size
+    if (int r = resize_pose_tables(c, kPoseCapInit, 0)) return r;
+  } else {
+    c->h_poses.assign((size_t)kPoseCapInit * 16, 0.0f);
+    for (uint32_t t = 0; t < kPoseCapInit; ++t)
+      for (int i = 0; i < 4; ++i) c->h_poses[16 * (size_t)t + 5 * i] = 1.0f;
+    c->h_poses_inv = c->h_poses;
+    SB_CUDA(c, cudaMemcpyAsync(c->poses, c->h_poses.data(), (size_t)kPoseCapInit * 64, cudaMemcpyHostToDevice, c->stream));
+    SB_CUDA(c, cudaMemcpyAsync(c->poses_inv, c->h_poses.data(), (size_t)kPoseCapInit * 64, cudaMemcpyHostToDevice,
+                               c->stream));
+  }
   SB_CUDA(c, cudaMemsetAsync(c->res->counts, 0, sizeof(c->res->counts), c->stream));
   c->timestamp = 0;
   ident_d(c->currentPose); ident_d(c->lastPose); ident_d(c->currentPose_old); ident_d(c->currentPose_new);
@@ -438,10 +518,10 @@ int alloc_buffers(sb_ctx* c) {
   SB_CUDA(c, cudaMemsetAsync(c->lb_desc, 0, (nb + 16) * 8, c->stream));
   SB_CUDA(c, dev_alloc(c->lb_ticket, 64));
   SB_CUDA(c, cudaMemsetAsync(c->lb_ticket, 0, 64, c->stream));
-  SB_CUDA(c, dev_alloc(c->poses, (size_t)kMaxPoses * 64));
-  SB_CUDA(c, dev_alloc(c->poses_inv, (size_t)kMaxPoses * 64));
-  SB_CUDA(c, dev_alloc(c->Mtab_old, (size_t)kMaxPoses * 64));
-  SB_CUDA(c, dev_alloc(c->Mtab_new, (size_t)kMaxPoses * 64));
+  SB_CUDA(c, dev_alloc(c->poses, (size_t)c->pose_cap * 64));
+  SB_CUDA(c, dev_alloc(c->poses_inv, (size_t)c->pose_cap * 64));
+  SB_CUDA(c, dev_alloc(c->Mtab_old, (size_t)c->pose_cap * 64));
+  SB_CUDA(c, dev_alloc(c->Mtab_new, (size_t)c->pose_cap * 64));
   SB_CUDA(c, dev_alloc(c->key_old, Pm * 8 * 3));
   c->key_new = c->key_old + Pm;
   c->key_comp = c->key_old + 2 * Pm;
@@ -471,14 +551,22 @@ uint32_t n_live(const sb_ctx* c) { return c->n_host - c->n_holes; }
 
 int t_threshold(const sb_ctx* c) { return (int)(c->map_timestamp - kComposeAge); }  // SurfelMap.cpp:873 (Q9)
 
-uint32_t pose_table_count(const sb_ctx* c) {
-  uint32_t n = c->map_timestamp + 1;
-  return n < kMaxPoses ? n : kMaxPoses;
+// One past the last entry of the product tables: the entry of the map's next scan and every entry a surfel refers to.
+uint32_t pose_window_end(const sb_ctx* c) {
+  const uint64_t n = std::max<uint64_t>((uint64_t)c->map_timestamp + 1, c->pose_ref_end);
+  return n < c->pose_cap ? (uint32_t)n : c->pose_cap;
 }
 
+// out[t] = A * poses[t] over the entries the live surfels can refer to (entries outside hold stale products, unread)
+void pose_products(sb_ctx* c, const Launch& L, const float* A, const Mat4* A_dev, float* out) {
+  const uint32_t end = pose_window_end(c);
+  launch_pose_products(L, mat4_from(A), A_dev, c->poses, out, std::min(c->pose_ref_begin, end), end);
+}
+
+// (callers grow the table first: reserve_poses)
 int set_pose_entry(sb_ctx* c, uint32_t t, const float* pose) {
+  if (t >= c->pose_cap) return fail(c, SB_ERR_CAPACITY, "pose table: entry beyond the table");
   c->map_version += 1;
-  if (t >= kMaxPoses) return fail(c, SB_ERR_CAPACITY, "pose table full (10000 poses, SurfelMap.h:205)");
   memcpy(&c->h_poses[16 * (size_t)t], pose, 64);
   sbg::rigid_inverse_f(pose, &c->h_poses_inv[16 * (size_t)t]);
   SB_CUDA(c, cudaMemcpyAsync(c->poses + 16 * (size_t)t, &c->h_poses[16 * (size_t)t], 64, cudaMemcpyHostToDevice, c->stream));
@@ -525,12 +613,11 @@ int render_full(sb_ctx* c, const float* pose_old, const float* pose_new, float c
     sbg::rigid_inverse_f(pose_new, inv_new);
   }
   const bool same = inv_dev != nullptr || memcmp(pose_old, pose_new, 64) == 0;
-  uint32_t np = pose_table_count(c);
   // table_ready: Mtab_old already holds inv(pose) * poseTable from the map update of this scan (same pose)
-  if (!table_ready) launch_pose_products(L, mat4_from(inv_old), inv_dev, c->poses, c->Mtab_old, np);
+  if (!table_ready) pose_products(c, L, inv_old, inv_dev, c->Mtab_old);
   float* Mnew = c->Mtab_old;
   if (!same) {
-    launch_pose_products(L, mat4_from(inv_new), nullptr, c->poses, c->Mtab_new, np);
+    pose_products(c, L, inv_new, nullptr, c->Mtab_new);
     Mnew = c->Mtab_new;
   }
   if (c->p.compose_rendering) {
@@ -572,7 +659,7 @@ int render_single(sb_ctx* c, const float* pose, float conf_thr, int which, const
   size_t Pm = (size_t)kp.Wm * kp.Hm;
   float inv[16] = {0};
   if (pose) sbg::rigid_inverse_f(pose, inv);
-  if (!table_ready) launch_pose_products(L, mat4_from(inv), inv_dev, c->poses, c->Mtab_old, pose_table_count(c));
+  if (!table_ready) pose_products(c, L, inv, inv_dev, c->Mtab_old);
   unsigned long long* key = which ? c->key_new : c->key_old;
   RenderTargets t{which ? nullptr : key, which ? key : nullptr, nullptr};
   launch_render_scatter(L, kp, c->A, c->res->counts, c->live, n_grid(c), c->Mtab_old, conf_thr, t_threshold(c), which ? 0 : 1,
@@ -837,6 +924,7 @@ int append_tiles(sb_ctx* c, int32_t i0, int32_t j0, int di, int dj) {  // Surfel
   }
   if (appended) {
     c->map_version += 1;
+    lower_pose_ref(c);
     SB_CUDA(c, cudaMemcpyAsync(c->res->counts, &c->n_host, 4, cudaMemcpyHostToDevice, c->stream));
     SB_CUDA(c, cudaStreamSynchronize(c->stream));  // the copy reads a member of the context: keep it ordered
   }
@@ -992,7 +1080,13 @@ int extract_surfels(sb_ctx* c, bool partially) {
     uint32_t slot = pg.n_slots++;
     // extractions can follow each other with no per-pixel prologue in between to clear the group totals
     SB_CUDA(c, cudaMemsetAsync(c->group_counts, 0, kGroupCounts * 4, c->stream));
-    launch_extract_to_pool(L, c->A, c->res->counts, c->live, c->n_host, c->poses, ctr, c->p.submap_extent, c->keep,
+    if (!c->pose_min_pending) {  // the passes lower counts[8]; the results of the next scan carry it back
+      SB_CUDA(c, cudaMemsetAsync(c->res->counts + 8, 0xff, 4, c->stream));
+      c->pose_min_pending = true;
+      c->pose_min_floor = c->map_timestamp;
+    }
+    launch_extract_to_pool(L, c->A, c->res->counts, c->live, c->n_host, c->poses, c->pose_cap, c->res->counts + 8, ctr,
+                           c->p.submap_extent, c->keep,
                            c->block_counts, c->group_counts, pg.pool, pg.setting.pool_cap, pg.d_rec, slot, kExtractCap);
     pg.tiles[idx] = slot;  // a tile extracted again replaces its cache entry (the old pool range is abandoned)
     if (partially) break;
@@ -1039,14 +1133,12 @@ int map_update(sb_ctx* c, const float* pose, const sb_frame* frame, const Mat4* 
   // the operator-level update works on the compacted map: its index map (sb_map_update_debug) indexes the surfels in order
   if (!deferred && (r = compact_map(c))) return r;
   if (!deferred) {
-    if (c->map_timestamp < kMaxPoses) {
-      if ((r = set_pose_entry(c, c->map_timestamp, pose))) return r;  // SurfelMap.cpp:494-495
-    }
+    if ((r = set_pose_entry(c, c->map_timestamp, pose))) return r;  // SurfelMap.cpp:494-495
     sbg::rigid_inverse_f(pose, inv_pose);  // :497
     memcpy(pose_h, pose, 64);
   }
   // K6a (table_ready: the Gauss-Newton kernel of this scan has already filled inv(pose) * poses[t])
-  if (!table_ready) launch_pose_products(L, mat4_from(inv_pose), inv_dev, c->poses, c->Mtab_old, pose_table_count(c));
+  if (!table_ready) pose_products(c, L, inv_pose, inv_dev, c->Mtab_old);
   // K6b (+ index keys re-armed, integrated flags cleared) -- already done by the tiled preprocessing pass of this scan
   // when the frame is the one it produced
   if (!(c->prepped_for_update && frame == c->cur)) launch_radius(L, kp, frame->d, c->radius_map, c->key_index, c->integrated, c->group_counts);
@@ -1086,14 +1178,14 @@ int map_update(sb_ctx* c, const float* pose, const sb_frame* frame, const Mat4* 
                      c->res->counts);
   uint64_t up = (uint64_t)n_grid(c) + Pd;  // the map can grow by at most one surfel per pixel
   c->n_upper = up > kMaxSurfels ? kMaxSurfels : (uint32_t)up;
-  const uint32_t entry = c->map_timestamp < kMaxPoses ? c->map_timestamp : kMaxPoses - 1;  // of the new surfels
-  if (entry + 1 > c->pose_ref_end) c->pose_ref_end = entry + 1;
+  if (c->map_timestamp + 1 > c->pose_ref_end) c->pose_ref_end = c->map_timestamp + 1;  // the entry of the new surfels
   if (deferred) {
     c->map_timestamp += 1;
     return SB_OK;
   }
-  uint32_t cnt[4];
-  if ((r = fetch_counts(c, cnt, 4))) return r;
+  uint32_t cnt[9];
+  if ((r = fetch_counts(c, cnt, 9))) return r;
+  absorb_pose_min(c, cnt[8]);
   c->n_host = cnt[0];
   c->n_holes = 0;  // (dense)
   c->n_upper = cnt[0];
@@ -1237,9 +1329,8 @@ int render_composed_internal(sb_ctx* c, const float* pose_old, const float* pose
   float inv_old[16], inv_new[16];
   sbg::rigid_inverse_f(pose_old, inv_old);
   sbg::rigid_inverse_f(pose_new, inv_new);
-  uint32_t np = pose_table_count(c);
-  launch_pose_products(L, mat4_from(inv_old), nullptr, c->poses, c->Mtab_old, np);
-  launch_pose_products(L, mat4_from(inv_new), nullptr, c->poses, c->Mtab_new, np);
+  pose_products(c, L, inv_old, nullptr, c->Mtab_old);
+  pose_products(c, L, inv_new, nullptr, c->Mtab_new);
   RenderTargets t{nullptr, nullptr, c->key_comp};
   int thr = t_threshold(c);
   // GL_LEQUAL (SurfelMap.cpp:1126), old then new without clearing (:1146-1152); COLOR2 not attached (Q4)
@@ -1264,7 +1355,7 @@ int update_pose_enqueue(sb_ctx* c, bool* tables_ready, bool* index_fused) {
   *index_fused = false;
   int r;
   Launch L = L_(c);
-  const uint32_t np = pose_table_count(c);
+  const uint32_t pose_end = pose_window_end(c), pose_begin = std::min(c->pose_ref_begin, pose_end);
   int max_iter = p.max_iterations;
   if (max_iter <= 0 || max_iter > kMaxGnIter) max_iter = kMaxGnIter;
   const int r0 = c->comm_on ? c->row_begin : 0, r1 = c->comm_on ? c->row_end : c->kp.H;
@@ -1278,7 +1369,8 @@ int update_pose_enqueue(sb_ctx* c, bool* tables_ready, bool* index_fused) {
     job.pd = &c->res->pose;
     job.Mtab = c->Mtab_old;
     job.poses = c->poses;
-    job.n_poses = np;
+    job.pose_begin = pose_begin;
+    job.pose_end = pose_end;
     job.initialize_identity = p.initialize_identity;
     job.fallback_mode = p.fallback_mode;
     job.timestamp = c->timestamp;
@@ -1317,8 +1409,10 @@ int update_pose_enqueue(sb_ctx* c, bool* tables_ready, bool* index_fused) {
     post.poses = c->poses;
     post.poses_inv = c->poses_inv;
     post.t_map = c->map_timestamp;
+    post.pose_cap = c->pose_cap;
     post.Mtab = c->Mtab_old;
-    post.n_poses = np;
+    post.pose_begin = pose_begin;
+    post.pose_end = pose_end;
     post.fallback_mode = p.fallback_mode;
     post.timestamp = c->timestamp;
     post.max_iter = max_iter;
@@ -1359,7 +1453,7 @@ int update_pose_enqueue(sb_ctx* c, bool* tables_ready, bool* index_fused) {
         return r;
     }
   }
-  launch_pose_finalize(L, c->gn2, &c->res->pose, 1, c->poses, c->poses_inv, c->map_timestamp);
+  launch_pose_finalize(L, c->gn2, &c->res->pose, 1, c->poses, c->poses_inv, c->map_timestamp, c->pose_cap);
   return SB_OK;
 }
 
@@ -1840,8 +1934,9 @@ int sb_map_update(sb_ctx* c, const float pose[16], const sb_frame* frame) {
   if (!c || !pose || !frame) return fail(c, SB_ERR_INVALID, "map_update: null argument");
   if (frame->d.W != c->kp.W || frame->d.H != c->kp.H) return fail(c, SB_ERR_INVALID, "map_update: frame size mismatch");
   cudaSetDevice(c->device);
-  int r = map_update(c, pose, frame);
+  int r = reserve_poses(c, (uint64_t)c->map_timestamp + 1);  // the entry this update writes
   if (r) return r;
+  if ((r = map_update(c, pose, frame))) return r;
   SB_CUDA(c, cudaGetLastError());
   return SB_OK;
 }
@@ -1849,16 +1944,26 @@ int sb_map_update(sb_ctx* c, const float pose[16], const sb_frame* frame) {
 int sb_map_update_poses(sb_ctx* c, const float* poses16, uint32_t count) {
   if (!c || (!poses16 && count)) return SB_ERR_INVALID;
   cudaSetDevice(c->device);
-  for (uint32_t t = 0; t < count && t < kMaxPoses; ++t) {
-    int r = set_pose_entry(c, t, poses16 + 16 * (size_t)t);
-    if (r) return r;
-  }
+  int r = reserve_poses(c, count);
+  if (r) return r;
+  for (uint32_t t = 0; t < count; ++t)
+    if ((r = set_pose_entry(c, t, poses16 + 16 * (size_t)t))) return r;
   return SB_OK;
 }
 int sb_map_set_pose(sb_ctx* c, uint32_t t, const float pose[16]) {
   if (!c || !pose) return SB_ERR_INVALID;
   cudaSetDevice(c->device);
+  int r = reserve_poses(c, (uint64_t)t + 1);
+  if (r) return r;
   return set_pose_entry(c, t, pose);
+}
+int sb_pose_table_info(sb_ctx* c, uint32_t* capacity, uint32_t* begin, uint32_t* end) {
+  if (!c) return SB_ERR_INVALID;
+  const uint32_t e = pose_window_end(c);
+  if (capacity) *capacity = c->pose_cap;
+  if (begin) *begin = std::min(c->pose_ref_begin, e);
+  if (end) *end = e;
+  return SB_OK;
 }
 int sb_map_size(sb_ctx* c, uint32_t* n) {
   if (!c || !n) return SB_ERR_INVALID;
@@ -1888,16 +1993,26 @@ int sb_map_upload(sb_ctx* c, const sb_surfel* src, uint32_t n, uint32_t timestam
   if (!c || (!src && n)) return SB_ERR_INVALID;
   if (n > kMaxSurfels) return fail(c, SB_ERR_CAPACITY, "map_upload: more than 4194304 surfels");
   cudaSetDevice(c->device);
+  // the pose-table entry of each surfel, as pose_index() reads it from the count field; the table grows to hold them all
+  uint32_t e_min = timestamp, e_max = 0;
+  for (uint32_t i = 0; i < n; ++i) {
+    const float t = src[i].count;
+    if (t >= (float)kPoseCapMax)
+      return fail(c, SB_ERR_CAPACITY, "map_upload: surfel " + std::to_string(i) + " refers to a pose-table entry beyond "
+                                      "the last one, 16777215");
+    const uint32_t e = !(t >= 1.0f) ? 0u : (uint32_t)t;
+    e_min = std::min(e_min, e);
+    e_max = std::max(e_max, e);
+  }
+  int r = reserve_poses(c, n ? (uint64_t)e_max + 1 : 0);
+  if (r) return r;
   if (n) {
     SB_CUDA(c, cudaMemcpyAsync(c->T.p0, src, (size_t)n * 64, cudaMemcpyHostToDevice, c->stream));
     launch_aos_to_soa(L_(c), reinterpret_cast<const sb_surfel*>(c->T.p0), c->A, 0, n);
     SB_CUDA(c, cudaMemsetAsync(c->live, 1, n, c->stream));
   }
-  for (uint32_t i = 0; i < n; ++i) {  // the pose-table entry of each surfel, as pose_index() reads it from the count field
-    const float t = src[i].count;
-    const uint32_t e = !(t >= 1.0f) ? 0u : t >= (float)(kMaxPoses - 1) ? kMaxPoses - 1 : (uint32_t)t;
-    if (e + 1 > c->pose_ref_end) c->pose_ref_end = e + 1;
-  }
+  if (n && e_max + 1 > c->pose_ref_end) c->pose_ref_end = e_max + 1;
+  lower_pose_ref(c, e_min);  // the map is replaced: its oldest surfel, or the entries the next scans create
   c->n_host = n;
   c->n_holes = 0;  // (overwritten: nothing to compact)
   c->n_upper = n;
@@ -1982,6 +2097,7 @@ int sb_process_scan_timed(sb_ctx* c, const float* pts4, const float* labels, con
   const float4* dp; const float* dl; const float* dq;
   int r = upload_scan(c, pts4, labels, probs, n, on_device, &dp, &dl, &dq);
   if (r) return r;
+  if ((r = reserve_poses(c, (uint64_t)c->map_timestamp + 1))) return r;  // the entry this scan writes
   // deskewing with the motion the next Gauss-Newton run starts from: lastIncrement_ as the previous scan left it
   DeskewArgs da;
   bool deskew = false;
@@ -2013,7 +2129,7 @@ int sb_process_scan_timed(sb_ctx* c, const float* pts4, const float* labels, con
       loop_ran = true;
     }
   } else {
-    launch_pose_finalize(L, c->gn2, &c->res->pose, 0, c->poses, c->poses_inv, c->map_timestamp);
+    launch_pose_finalize(L, c->gn2, &c->res->pose, 0, c->poses, c->poses_inv, c->map_timestamp, c->pose_cap);
   }
   // updateMap(), :797-804
   const uint32_t t_map = c->map_timestamp;
@@ -2037,13 +2153,13 @@ int sb_process_scan_timed(sb_ctx* c, const float* pts4, const float* labels, con
   c->n_upper = rb.counts[0];
   c->n_updated = rb.counts[2];
   c->n_new = rb.counts[3];
+  absorb_pose_min(c, rb.counts[8]);
   if (rb.pose.gn_error) return gn_fail(c);
   if (!loop_ran) absorb_pose_block(c, rb, had_icp);  // (the loop-closure step has already done it, and chose currentPose_old_)
   const Mat4 P_cur = rb.pose.P_cur;
-  if (t_map < kMaxPoses) {  // host mirror of the pose table entry written by k_pose_finalize
-    memcpy(&c->h_poses[16 * (size_t)t_map], P_cur.m, 64);
-    sbg::rigid_inverse_f(P_cur.m, &c->h_poses_inv[16 * (size_t)t_map]);
-  }
+  // host mirror of the pose table entry written by k_pose_finalize
+  memcpy(&c->h_poses[16 * (size_t)t_map], P_cur.m, 64);
+  sbg::rigid_inverse_f(P_cur.m, &c->h_poses_inv[16 * (size_t)t_map]);
   if (p.render_after_update)  // the render's memo entry, now that the pose bits are known on the host
     c->memo.store(memo_key(c, P_cur.m, P_cur.m, ct2, c->cur_model));
   // submap paging (SurfelMap.cpp:547, 744-824) with the pose now known on the host. Re-inserting cached tiles changes
@@ -2195,12 +2311,14 @@ int sb_integrate_loop_closures(sb_ctx* c, const double* poses16, uint32_t n, uin
   memcpy(cur.m, c->currentPose, 128);
   memcpy(cold.m, c->currentPose_old, 128);
   memcpy(cnew.m, c->currentPose_new, 128);
+  // the poses go into the pose table: grow it before anything changes
+  int r = reserve_poses(c, std::max<uint64_t>(opt.size(), S.graph.poses.size()));
+  if (r) return r;
   std::vector<lp::M4> all = S.integrate(opt, cur, cold, cnew);
   if (all.empty()) return fail(c, SB_ERR_STATE, "integrate_loop_closures: no optimisation request pending");
   std::vector<float> pf(all.size() * 16);
   for (size_t t = 0; t < all.size(); ++t) lp::to_float(all[t], &pf[16 * t]);
-  int r = sb_map_update_poses(c, pf.data(), (uint32_t)all.size());  // map_->updatePoses(casted_poses)   :232
-  if (r) return r;
+  if ((r = sb_map_update_poses(c, pf.data(), (uint32_t)all.size()))) return r;  // map_->updatePoses(casted_poses)   :232
   memcpy(c->currentPose_old, cold.m, 128);  // currentPose_new_ = currentPose_old_ = currentPose_   :240
   memcpy(c->currentPose_new, cnew.m, 128);
   if ((r = sb_set_current_pose(c, cur.m))) return r;  // currentPose_ = difference * currentPose_   :236 (host + device copy)
@@ -2535,6 +2653,7 @@ struct StateImage {
   double stats[16];
   uint32_t cur_has_semantics = 0, last_has_semantics = 0, close_loops = 0;
   uint32_t n_live = 0, map_timestamp = 0, pose_ref_end = 0, n_updated = 0, n_new = 0;
+  uint32_t pose_cap = kPoseCapInit;     // entries of the pose tables
   std::vector<float> poses, poses_inv;  // the used entries of the device pose tables
   ResultBlock result;
   lp::State loop;
@@ -2574,7 +2693,7 @@ lp::OptResult get_result(Reader& r) {
 
 void write_header(Writer& w, const StateImage& s, uint64_t total) {
   w.bytes(kStateMagic, 8);
-  w.put(kStateFormat); w.put((uint32_t)SB_VERSION); w.put((uint32_t)sizeof(sb_surfel)); w.put(kMaxPoses);
+  w.put(kStateFormat); w.put((uint32_t)SB_VERSION); w.put((uint32_t)sizeof(sb_surfel)); w.put(s.pose_cap);
   w.put(s.p.data_width); w.put(s.p.data_height); w.put(s.p.model_width); w.put(s.p.model_height);
   w.put(total);
 #define X(f) w.put(s.p.f);
@@ -2688,7 +2807,9 @@ const char* read_host(Reader& r, const sb_ctx* c, StateImage& s) {
   if (!r.ok) return "truncated header";
   if (fmt != kStateFormat) return "unsupported checkpoint format version";
   if (ver != SB_VERSION) return "checkpoint written by another library version (SB_VERSION)";
-  if (ssz != sizeof(sb_surfel) || mp != kMaxPoses) return "checkpoint written with another surfel size / pose capacity";
+  if (ssz != sizeof(sb_surfel) || mp < kPoseCapInit || mp > kPoseCapMax)
+    return "checkpoint written with another surfel size / pose capacity";
+  s.pose_cap = mp;
   int32_t dims[4];
   for (int32_t& d : dims) d = r.get<int32_t>();
   const uint64_t total = r.get<uint64_t>();
@@ -2735,7 +2856,7 @@ const char* read_host(Reader& r, const sb_ctx* c, StateImage& s) {
   if (!read_close(r, start, len)) return "malformed state section";
   // A digest is no signature: every field that later sizes a copy or indexes device memory is range-checked here.
   if (s.n_live > kMaxSurfels) return "checkpoint exceeds the map / tile-pool capacity";
-  if (s.pose_ref_end > kMaxPoses) return "malformed map state (pose-table reference beyond the table)";
+  if (s.pose_ref_end > s.pose_cap) return "malformed map state (pose-table reference beyond the table)";
 
   len = read_open(r, S_LOOP);
   start = r.off;
@@ -2773,7 +2894,7 @@ const char* read_host(Reader& r, const sb_ctx* c, StateImage& s) {
   len = read_open(r, S_POSES);
   start = r.off;
   const uint32_t np = r.count(128);
-  if (np > kMaxPoses) return "malformed pose tables";
+  if (np > s.pose_cap) return "malformed pose tables";
   s.poses.resize((size_t)np * 16);
   s.poses_inv.resize((size_t)np * 16);
   r.bytes(s.poses.data(), s.poses.size() * 4);
@@ -2969,8 +3090,9 @@ int capture(sb_ctx* c, StateImage& s) {
   s.n_updated = c->n_updated; s.n_new = c->n_new;
   if (int r = capture_paging(c, s.paging)) return r;
   // the used entries of the pose tables: those the map can refer to, and any set beyond them through sb_map_set_pose
-  uint32_t np = pose_table_count(c);
-  for (uint32_t t = kMaxPoses; t > np; --t) {
+  s.pose_cap = c->pose_cap;
+  uint32_t np = (uint32_t)std::min<uint64_t>((uint64_t)c->map_timestamp + 1, c->pose_cap);
+  for (uint32_t t = c->pose_cap; t > np; --t) {
     const float* e = &c->h_poses[16 * (size_t)(t - 1)];
     bool ident = true;
     for (int i = 0; i < 16; ++i) ident = ident && e[i] == ((i % 5 == 0) ? 1.0f : 0.0f);
@@ -2983,6 +3105,7 @@ int capture(sb_ctx* c, StateImage& s) {
   SB_CUDA(c, cudaMemcpy(&s.result, c->res, sizeof(ResultBlock), cudaMemcpyDeviceToHost));
   s.result.counts[0] = s.n_live;  // the map is restored dense: its physical end is the live count, no dead slots
   s.result.counts[5] = 0;
+  s.result.counts[8] = 0;  // (the extraction passes' pending minimum: a loaded context starts from bound 0)
   s.loop = c->loop;
   s.deskew = c->deskew;
   return SB_OK;
@@ -3012,16 +3135,18 @@ int apply(sb_ctx* c, const StateImage& s) {
   c->n_host = s.n_live; c->n_holes = 0; c->lazy_update = false; c->n_upper = s.n_live;
   c->prepped_for_update = false;
   c->map_timestamp = s.map_timestamp; c->pose_ref_end = s.pose_ref_end;
+  lower_pose_ref(c);
   c->n_updated = s.n_updated; c->n_new = s.n_new;
-  c->h_poses.assign((size_t)kMaxPoses * 16, 0.0f);
-  for (uint32_t t = 0; t < kMaxPoses; ++t)
+  // (the tables already have the checkpoint's size: sb_state_load resized them)
+  const uint32_t cap = c->pose_cap;
+  c->h_poses.assign((size_t)cap * 16, 0.0f);
+  for (uint32_t t = 0; t < cap; ++t)
     for (int i = 0; i < 4; ++i) c->h_poses[16 * (size_t)t + 5 * i] = 1.0f;
   c->h_poses_inv = c->h_poses;
   memcpy(c->h_poses.data(), s.poses.data(), s.poses.size() * 4);
   memcpy(c->h_poses_inv.data(), s.poses_inv.data(), s.poses_inv.size() * 4);
-  SB_CUDA(c, cudaMemcpyAsync(c->poses, c->h_poses.data(), (size_t)kMaxPoses * 64, cudaMemcpyHostToDevice, c->stream));
-  SB_CUDA(c, cudaMemcpyAsync(c->poses_inv, c->h_poses_inv.data(), (size_t)kMaxPoses * 64, cudaMemcpyHostToDevice,
-                             c->stream));
+  SB_CUDA(c, cudaMemcpyAsync(c->poses, c->h_poses.data(), (size_t)cap * 64, cudaMemcpyHostToDevice, c->stream));
+  SB_CUDA(c, cudaMemcpyAsync(c->poses_inv, c->h_poses_inv.data(), (size_t)cap * 64, cudaMemcpyHostToDevice, c->stream));
   c->host->result = s.result;
   SB_CUDA(c, cudaMemcpyAsync(c->res, &c->host->result, sizeof(ResultBlock), cudaMemcpyHostToDevice, c->stream));
   const std::vector<uint2>& rec = s.paging.rec.v;
@@ -3142,6 +3267,8 @@ int sb_state_load(sb_ctx* c, const void* src, uint64_t n) {
     rd.off += len;
   }
   if (rd.n - rd.off != 8) return fail(c, SB_ERR_INVALID, "state_load: checkpoint size does not match its sections");
+  // the pose tables take the checkpoint's size (no change when the allocation fails)
+  if (s.pose_cap != c->pose_cap && (r = resize_pose_tables(c, s.pose_cap, 0))) return r;
   // ---- the header is sound: from here on the context changes ----
   if ((r = discard_prefetch(c))) return r;
   if ((r = state_staging(c))) return r;

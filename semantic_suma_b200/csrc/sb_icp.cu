@@ -306,7 +306,7 @@ __device__ void pose_after_icp_body(const double* gn_pose, int gn_k, PoseDev* pd
 // lastPose_ = currentPose_; currentPose_ = currentPose_ * increment; ... (SurfelMapping.cpp:451-473) and the pose-table
 // entry of this scan (SurfelMap.cpp:494-495)
 __device__ void pose_finalize_body(const double* recovery_pose, PoseDev* pd, int had_icp, float* poses, float* poses_inv,
-                                   uint32_t t) {
+                                   uint32_t t, uint32_t pose_cap) {
   if (had_icp) {
     double inc[16], np[16];
     if (pd->fallback)
@@ -323,7 +323,7 @@ __device__ void pose_finalize_body(const double* recovery_pose, PoseDev* pd, int
   }
   for (int i = 0; i < 16; ++i) pd->P_cur.m[i] = (float)pd->currentPose[i];
   sbg::rigid_inverse_f(pd->P_cur.m, pd->invP_cur.m);
-  if (t < kMaxPoses) {
+  if (t < pose_cap) {  // (the host grows the table before it enqueues the scan)
     float inv[16];
     sbg::rigid_inverse_f(pd->P_cur.m, inv);
     for (int i = 0; i < 16; ++i) {
@@ -368,15 +368,15 @@ void launch_pose_after_icp(const Launch& L, const GnState* gn, PoseDev* pd, cons
 }
 
 __global__ void k_pose_finalize(const GnState* __restrict__ gn, PoseDev* __restrict__ pd, int had_icp,
-                                float* __restrict__ poses, float* __restrict__ poses_inv, uint32_t t) {
+                                float* __restrict__ poses, float* __restrict__ poses_inv, uint32_t t, uint32_t pose_cap) {
   if (threadIdx.x != 0) return;
-  pose_finalize_body(gn->pose, pd, had_icp, poses, poses_inv, t);
+  pose_finalize_body(gn->pose, pd, had_icp, poses, poses_inv, t, pose_cap);
 }
 void launch_pose_finalize(const Launch& L, const GnState* gn, PoseDev* pd, int had_icp, float* poses, float* poses_inv,
-                          uint32_t t) {
+                          uint32_t t, uint32_t pose_cap) {
   {
     ScopedKernel sk(L, K_GN_INIT);
-    k_pose_finalize<<<1, 32, 0, L.stream>>>(gn, pd, had_icp, poses, poses_inv, t);
+    k_pose_finalize<<<1, 32, 0, L.stream>>>(gn, pd, had_icp, poses, poses_inv, t, pose_cap);
   }
 }
 
@@ -798,7 +798,7 @@ __global__ void __launch_bounds__(kIcpThreads, 2) k_gn_persistent(KParams kp, Gn
           for (int i = 0; i < 16; ++i) T0[i] = job.initialize_identity ? ((i % 5 == 0) ? 1.0 : 0.0) : pd->lastIncrement[i];
           pose_after_icp_body(sh.P, st->k, pd, T0, job.timestamp, job.fallback_mode);
         } else if (job.mode == GN_POST) {
-          pose_finalize_body(st->pose, pd, 1, job.poses, job.poses_inv, job.t_map);
+          pose_finalize_body(st->pose, pd, 1, job.poses, job.poses_inv, job.t_map, job.pose_cap);
         }
       }
       if (lane == 0) {
@@ -829,14 +829,17 @@ __global__ void __launch_bounds__(kIcpThreads, 2) k_gn_persistent(KParams kp, Gn
       if (!done) clear_replicas(my_slots, lane);  // behind the release, see above
     }
   }
-  // ---- all blocks: the table inv(P) * poses[t] of the rendering / map update that follows (render_surfels.vert:46) ----
+  // ---- all blocks: the table inv(P) * poses[t] of the rendering / map update that follows (render_surfels.vert:46), over
+  // the entries the live surfels can refer to ----
   if (job.Mtab) {
     if (*(volatile int*)&pd->gn_error) return;
     const float* A = job.mode == GN_MAIN ? pd->invP_active.m : pd->invP_cur.m;
     float a[16];
 #pragma unroll
     for (int i = 0; i < 16; ++i) a[i] = *(volatile const float*)&A[i];
-    for (uint32_t t = blockIdx.x * blockDim.x + threadIdx.x; t < job.n_poses; t += gridDim.x * blockDim.x) {
+    const uint32_t t0 = job.pose_begin, nt = job.pose_end - job.pose_begin;
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < nt; i += gridDim.x * blockDim.x) {
+      const uint32_t t = t0 + i;
       float b[16], c[16];
       load_mat_cg(job.poses, (int)t, b);
       mat4_mul<float>(a, b, c);

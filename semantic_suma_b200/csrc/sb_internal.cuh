@@ -16,7 +16,10 @@
 namespace sb {
 
 constexpr uint32_t kMaxSurfels = 2048u * 2048u;  // SurfelMap.h:87
-constexpr uint32_t kMaxPoses = 10000u;           // SurfelMap.h:205
+// The pose table starts at the reference's fixed size (SurfelMap.h:205) and doubles on demand up to 2^24 entries: a
+// surfel keeps its entry in the float `count` field, which holds integers exactly only up to 2^24 (DESIGN.md section 12).
+constexpr uint32_t kPoseCapInit = 10000u;
+constexpr uint32_t kPoseCapMax = 1u << 24;
 constexpr uint32_t kExtractCap = 500000u;        // SurfelMap.cpp:279
 constexpr uint32_t kComposeAge = 100u;           // SurfelMap.h:144
 constexpr int kMaxGnIter = 256;
@@ -38,6 +41,7 @@ struct KParams {
   float pixel_size, min_radius, max_radius, radconf_angle_thresh, update_angle_thresh, map_max_distance;
   float max_loop_closure_distance;
   int label_offset_quirk;
+  uint32_t pose_cap;  // entries of the pose tables (pose_index() clamps to it: malformed input only)
 };
 
 // Frame.h:21-79: three RGBA32F images; one allocation, SoA of images
@@ -122,7 +126,7 @@ struct ResultBlock {
   char pad1[8192 - 4096 - 64 * sizeof(long long)];
   // [0] physical end of the surfel slots, [1] physical end after the update (base for new), [2] kept updated,
   // [3] kept new, [4] extracted, [5] dead slots below [1] after an in-place update, [6] / [7] end of the written range /
-  // number kept of a compaction of the map (not read back)
+  // number kept of a compaction of the map (not read back), [8] smallest pose-table entry the extraction passes saw
   uint32_t counts[16];
 };
 static_assert(offsetof(ResultBlock, sums) == 4096, "result block layout");
@@ -237,8 +241,9 @@ struct GnJob {
   GnState* st;  // state of the run (GN_PLAIN: prepared by k_gn_init)
   PoseDev* pd;  // GN_MAIN / GN_POST
   long long* stats32;                       // GN_POST: raw sums of the statistics pass, read by the host after the scan
-  float* poses; float* poses_inv; uint32_t t_map;  // GN_POST: pose-table entry of this scan
-  float* Mtab; uint32_t n_poses;            // GN_MAIN / GN_POST: table inv(P) * poses[t] filled at the end (or null)
+  float* poses; float* poses_inv; uint32_t t_map, pose_cap;  // GN_POST: pose-table entry of this scan, table size
+  // GN_MAIN / GN_POST: table inv(P) * poses[t] filled at the end over the window [pose_begin, pose_end) (or null)
+  float* Mtab; uint32_t pose_begin, pose_end;
   int initialize_identity, fallback_mode;
   uint32_t timestamp;
   int max_iter;
@@ -253,7 +258,7 @@ int gn_persistent_max_blocks(int sm_count);
 void launch_pose_after_icp(const Launch& L, const GnState* gn, PoseDev* pd, const Mat4d& T0, uint32_t timestamp,
                            int fallback_mode);
 void launch_pose_finalize(const Launch& L, const GnState* gn, PoseDev* pd, int had_icp, float* poses, float* poses_inv,
-                          uint32_t t);
+                          uint32_t t, uint32_t pose_cap);
 int icp_grid_blocks(int sm_count);
 int icp_balanced_blocks(int pixels, int max_blocks);
 
@@ -271,8 +276,9 @@ struct IndexFuse {
   const int* fallback;       // PoseDev::fallback of the scan: set -> no keys here, the gated index pass writes them all
   int same_projection;       // model and data projection parameters are bitwise equal: the render's projection serves
 };
+// out[t] = A * poses[t] for t in [begin, end): the entries the live surfels of the map can refer to
 void launch_pose_products(const Launch& L, const Mat4& A, const Mat4* A_dev, const float* poses, float* out,
-                          uint32_t count);
+                          uint32_t begin, uint32_t end);
 // Surfel slots [0, counts[0]) of the map; a slot whose liveness byte is 0 holds a surfel removed by an in-place update.
 // index != null: also write the index keys (IndexFuse).
 void launch_render_scatter(const Launch& L, const KParams& kp, SurfelPlanes s, const uint32_t* n_dev, const uint8_t* live,
@@ -312,9 +318,11 @@ void launch_gen_compact(const Launch& L, const KParams& kp, FrameDev frame, cons
                         float submap_extent, SurfelPlanes map, uint8_t* live, const uint32_t* lazy_groups,
                         unsigned long long* desc, uint32_t* ticket, uint32_t gen, uint32_t cap, uint32_t* counts);
 // the live surfels of one submap tile, in order, into pool slot `slot`: rec[slot] = {end of the slot in the pool, surfels
-// of the tile}; slot s starts at the end of slot s - 1. The group totals must be zero.
+// of the tile}; slot s starts at the end of slot s - 1. The group totals must be zero. *pose_min is lowered to the
+// smallest pose-table entry of the live surfels of the map (those of the tile included).
 void launch_extract_to_pool(const Launch& L, SurfelPlanes map, const uint32_t* n_dev, const uint8_t* live, uint32_t n_upper,
-                            const float* poses, float2 center, float extent, uint8_t* keep, uint32_t* block_counts,
+                            const float* poses, uint32_t pose_cap, uint32_t* pose_min, float2 center, float extent,
+                            uint8_t* keep, uint32_t* block_counts,
                             uint32_t* group_counts, SurfelPlanes pool, uint32_t pool_cap, uint2* rec, uint32_t slot,
                             uint32_t tile_cap);
 // Managed tile cache: dst[dst_base + d] = src[segs[i].x + d - segs[i].y] for d in [0, total), i the last segment with

@@ -31,11 +31,12 @@ const char* kernel_name(int id) {
   return (id >= 0 && id < K_COUNT) ? names[id] : "?";
 }
 
-__device__ __forceinline__ int pose_index(float count) {
+// a surfel's pose-table entry: its creation timestamp, kept in the count field; the clamp only catches malformed input
+// (the host grows the table before any entry at or beyond its size is referenced)
+__device__ __forceinline__ int pose_index(float count, uint32_t n_poses) {
   int c = (int)count;
   c = c < 0 ? 0 : c;
-  c = c >= (int)kMaxPoses ? (int)kMaxPoses - 1 : c;
-  return c;
+  return min(c, (int)n_poses - 1);
 }
 
 __device__ __forceinline__ void load_mat(const float* __restrict__ table, int idx, float* M) {
@@ -47,12 +48,12 @@ __device__ __forceinline__ void load_mat(const float* __restrict__ table, int id
   M[12] = d.x; M[13] = d.y; M[14] = d.z; M[15] = d.w;
 }
 
-// out[t] = A * poses[t]  (render_surfels.vert:46 evaluates (inv_pose * surfelPose) * v; the product is shared by all
-// surfels created at time t)
+// out[t] = A * poses[t] for t in [begin, end)  (render_surfels.vert:46 evaluates (inv_pose * surfelPose) * v; the product
+// is shared by all surfels created at time t)
 __global__ void k_pose_products(Mat4 A, const Mat4* __restrict__ A_dev, const float* __restrict__ poses,
-                                float* __restrict__ out, uint32_t count) {
-  uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= count) return;
+                                float* __restrict__ out, uint32_t begin, uint32_t end) {
+  uint32_t t = begin + blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= end) return;
   float a[16], b[16], c[16];
   for (int i = 0; i < 16; ++i) a[i] = A_dev ? A_dev->m[i] : A.m[i];
   load_mat(poses, (int)t, b);
@@ -61,11 +62,11 @@ __global__ void k_pose_products(Mat4 A, const Mat4* __restrict__ A_dev, const fl
 }
 
 void launch_pose_products(const Launch& L, const Mat4& A, const Mat4* A_dev, const float* poses, float* out,
-                          uint32_t count) {
-  if (count == 0) return;
+                          uint32_t begin, uint32_t end) {
+  if (end <= begin) return;
   {
     ScopedKernel sk(L, K_POSE_PRODUCTS);
-    k_pose_products<<<(count + 127) / 128, 128, 0, L.stream>>>(A, A_dev, poses, out, count);
+    k_pose_products<<<(end - begin + 127) / 128, 128, 0, L.stream>>>(A, A_dev, poses, out, begin, end);
   }
 }
 
@@ -385,7 +386,7 @@ __global__ void __launch_bounds__(kRenderThreads, kMinBlocks) k_render_scatter(K
   if (alive || indexed) {
     if (!kIndex) p0 = __ldg(s.p0 + k);
     float M[16];
-    load_mat(Mtab, pose_index(p2.w), M);
+    load_mat(Mtab, pose_index(p2.w, kp.pose_cap), M);
     V3 pp = xform_point(M, mk3(p0.x, p0.y, p0.z));
     V3 nn = xform_dir(M, mk3(p1.x, p1.y, p1.z));
     bool visible = dot3(nn, divs3(neg3(pp), len3(pp))) > 0.01f;  // .geom:84, the same test as gen_indexmap.vert
@@ -659,7 +660,8 @@ struct Px {
 };
 
 __device__ __forceinline__ Px resolve_px(const SurfelPlanes& s, unsigned long long key, const float* __restrict__ M_old,
-                                         const float* __restrict__ M_new, int fixed_pass, int lequal, bool need_semantic) {
+                                         const float* __restrict__ M_new, uint32_t n_poses, int fixed_pass, int lequal,
+                                         bool need_semantic) {
   Px o;
   o.v = o.n = o.s = make_float4(0.f, 0.f, 0.f, 0.f);
   if (key == ~0ull) return o;
@@ -673,7 +675,7 @@ __device__ __forceinline__ Px resolve_px(const SurfelPlanes& s, unsigned long lo
   if (fixed_pass >= 0) pass = fixed_pass;
   float4 p0 = __ldg(s.p0 + k), p1 = __ldg(s.p1 + k), p2 = __ldg(s.p2 + k);
   float M[16];
-  load_mat(pass ? M_new : M_old, pose_index(p2.w), M);
+  load_mat(pass ? M_new : M_old, pose_index(p2.w, n_poses), M);
   V3 pp = xform_point(M, mk3(p0.x, p0.y, p0.z));
   V3 nn = xform_dir(M, mk3(p1.x, p1.y, p1.z));
   o.v = make_float4(pp.x, pp.y, pp.z, 1.0f);  // render_surfels.frag:30, .geom:95-97 (flat: surfel centre)
@@ -695,7 +697,7 @@ __global__ void __launch_bounds__(kThreads) k_render_resolve(KParams kp, SurfelP
   if (t.key_old) {
     ko_raw = t.key_old[pix];
     t.key_old[pix] = ~0ull;
-    po = resolve_px(s, ko_raw, M_old, M_new, 0, 0, !keep_semantic);
+    po = resolve_px(s, ko_raw, M_old, M_new, kp.pose_cap, 0, 0, !keep_semantic);
     f_old.vertex[pix] = po.v;
     f_old.normal[pix] = po.n;
     if (!keep_semantic) f_old.semantic[pix] = po.s;
@@ -703,7 +705,7 @@ __global__ void __launch_bounds__(kThreads) k_render_resolve(KParams kp, SurfelP
   if (t.key_new) {
     kn_raw = t.key_new[pix];
     t.key_new[pix] = ~0ull;
-    pn = resolve_px(s, kn_raw, M_old, M_new, 1, 0, !keep_semantic);
+    pn = resolve_px(s, kn_raw, M_old, M_new, kp.pose_cap, 1, 0, !keep_semantic);
     f_new.vertex[pix] = pn.v;
     f_new.normal[pix] = pn.n;
     if (!keep_semantic) f_new.semantic[pix] = pn.s;
@@ -718,7 +720,7 @@ __global__ void __launch_bounds__(kThreads) k_render_resolve(KParams kp, SurfelP
     // union of both passes is the smaller of the two per-pass winners, depth first, then pass, then surfel index
     unsigned long long ko = ko_raw, kn = kn_raw;
     if (kn != ~0ull) kn |= (1ull << 32);
-    Px pc = resolve_px(s, ko < kn ? ko : kn, M_old, M_new, -1, 0, !keep_semantic);
+    Px pc = resolve_px(s, ko < kn ? ko : kn, M_old, M_new, kp.pose_cap, -1, 0, !keep_semantic);
     f_comp.vertex[pix] = pc.v;
     f_comp.normal[pix] = pc.n;
     if (!keep_semantic) f_comp.semantic[pix] = pc.s;
@@ -726,7 +728,7 @@ __global__ void __launch_bounds__(kThreads) k_render_resolve(KParams kp, SurfelP
   if (t.key_comp) {
     unsigned long long kc = t.key_comp[pix];
     t.key_comp[pix] = ~0ull;
-    Px pc = resolve_px(s, kc, M_old, M_new, -1, lequal, !keep_semantic);
+    Px pc = resolve_px(s, kc, M_old, M_new, kp.pose_cap, -1, lequal, !keep_semantic);
     f_comp.vertex[pix] = pc.v;
     f_comp.normal[pix] = pc.n;
     if (!keep_semantic) f_comp.semantic[pix] = pc.s;
@@ -772,7 +774,7 @@ __global__ void __launch_bounds__(kThreads) k_index_scatter(KParams kp, SurfelPl
     float4 p0 = __ldg(s.p0 + k), p1 = __ldg(s.p1 + k), p2 = __ldg(s.p2 + k);
     if (!lv) continue;
     float M[16];
-    load_mat(Mtab, pose_index(p2.w), M);
+    load_mat(Mtab, pose_index(p2.w, kp.pose_cap), M);
     V3 v = xform_point(M, mk3(p0.x, p0.y, p0.z));
     V3 nrm = xform_dir(M, mk3(p1.x, p1.y, p1.z));
     if (!(dot3(nrm, divs3(neg3(v), len3(v))) > 0.01f)) continue;
@@ -928,10 +930,10 @@ __device__ __forceinline__ V3 slerp(V3 v0, V3 v1, float weight) {  // update_sur
   return add3(scale3(w0, v0), scale3(w1, v1));
 }
 
-__device__ __forceinline__ bool submap_keep(const float* __restrict__ poses, float4 p0, float4 p2, float2 center,
-                                            float extent) {
+__device__ __forceinline__ bool submap_keep(const float* __restrict__ poses, uint32_t n_poses, float4 p0, float4 p2,
+                                            float2 center, float extent) {
   float M[16];
-  load_mat(poses, pose_index(p2.w), M);
+  load_mat(poses, pose_index(p2.w, n_poses), M);
   V3 w = xform_point(M, mk3(p0.x, p0.y, p0.z));
   if ((int)__float_as_uint(p2.x) < 0 || fabsf(w.x - center.x) > extent || fabsf(w.y - center.y) > extent) return false;
   return true;
@@ -971,8 +973,9 @@ __device__ __forceinline__ bool same_bits(float4 a, float4 b) {
 // kLazy = true (in place): a lane is stored back into src only if its bits changed, a surfel that is not kept is marked
 // dead in `live`, and nothing moves: counts[1] = the physical end (k_gen_compact appends behind it and sums the live
 // count from the group totals). Dead slots are skipped in both modes, so a dense pass also compacts the map.
+// (kThreads, 4): four resident blocks per SM, 64 registers; the in-place instance takes 66 without the bound
 template <bool kLazy>
-__global__ void __launch_bounds__(kThreads) k_update_surfels(KParams kp, SurfelPlanes src, SurfelPlanes tmp,
+__global__ void __launch_bounds__(kThreads, 4) k_update_surfels(KParams kp, SurfelPlanes src, SurfelPlanes tmp,
                                                             const uint32_t* n_dev, UpdateArgs ua,
                                                             FrameDev f, uint8_t* __restrict__ integrated,
                                                             uint8_t* __restrict__ live, uint8_t* __restrict__ keep,
@@ -1000,7 +1003,7 @@ __global__ void __launch_bounds__(kThreads) k_update_surfels(KParams kp, SurfelP
     int s_ts = (int)__float_as_uint(p2.x);
     int surfel_age = timestamp - s_ts;
     int creation = (int)p2.w;
-    int ci = pose_index(p2.w);
+    int ci = pose_index(p2.w, kp.pose_cap);
     float SP[16];
     load_mat(ua.poses, ci, SP);
     const float* POSE = ua.pose_dev ? ua.pose_dev->m : ua.pose.m;
@@ -1121,7 +1124,7 @@ __global__ void __launch_bounds__(kThreads) k_update_surfels(KParams kp, SurfelP
     }
     if (o1.w < kp.log_unstable && kp.use_stability) valid_out = false;
     if (valid_out && mark_integrated) integrated[dpix] = 1;
-    kept = valid_out && submap_keep(ua.poses, o0, o2, ua.submap_center, ua.submap_extent);
+    kept = valid_out && submap_keep(ua.poses, kp.pose_cap, o0, o2, ua.submap_center, ua.submap_extent);
     const float4 o3 = avg_prob_set ? make_float4(p3.x, p3.y, p3.z, avg_prob) : p3;
     if (!kLazy) {
       tmp.p0[k] = o0;
@@ -1179,7 +1182,7 @@ __global__ void __launch_bounds__(kThreads) k_gen_compact(KParams kp, FrameDev f
       o1 = make_float4(ng.x, ng.y, ng.z, conf);
       o2 = make_float4(__uint_as_float((uint32_t)timestamp), pack_rgb(0.0f, 0.0f, 1.0f), 1.0f, (float)timestamp);
       o3 = S;
-      kept = submap_keep(poses, o0, o2, center, extent);
+      kept = submap_keep(poses, kp.pose_cap, o0, o2, center, extent);
     }
   }
   uint32_t block_count;
@@ -1216,29 +1219,45 @@ __global__ void __launch_bounds__(kThreads) k_gen_compact(KParams kp, FrameDev f
 }
 
 // extract_surfels.vert:44-62: flags of the live surfels inside one submap tile; with poses == nullptr, of every live
-// surfel (the compaction of a map with dead slots)
+// surfel (the compaction of a map with dead slots). With poses, *pose_min is also lowered to the smallest pose-table entry
+// of the live surfels (a lower bound for the product window, DESIGN.md section 12): one atomic per block.
 __global__ void __launch_bounds__(kThreads) k_extract_flags(SurfelPlanes s, const uint32_t* __restrict__ n_dev,
                                                            const uint8_t* __restrict__ live,
-                                                           const float* __restrict__ poses, float2 center, float extent,
+                                                           const float* __restrict__ poses, uint32_t n_poses,
+                                                           uint32_t* __restrict__ pose_min, float2 center, float extent,
                                                            uint8_t* __restrict__ keep,
                                                            uint32_t* __restrict__ block_counts,
                                                            uint32_t* __restrict__ group_counts) {
+  __shared__ uint32_t s_min[kThreads / 32];
   uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
   bool kept = false;
+  uint32_t entry = 0xffffffffu;
   if (k < *n_dev) {
     if (live[k]) {
       kept = true;
       if (poses) {
         float4 p0 = __ldg(s.p0 + k), p2 = __ldg(s.p2 + k);
         float M[16];
-        load_mat(poses, pose_index(p2.w), M);
+        const int ci = pose_index(p2.w, n_poses);
+        entry = (uint32_t)ci;
+        load_mat(poses, ci, M);
         V3 w = xform_point(M, mk3(p0.x, p0.y, p0.z));
         kept = !(fabsf(w.x - center.x) > extent || fabsf(w.y - center.y) > extent);
       }
     }
     keep[k] = kept ? 1 : 0;
   }
-  publish_block_count(kept, block_counts, group_counts);
+  if (poses) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) entry = min(entry, __shfl_xor_sync(0xffffffffu, entry, o));
+    if ((threadIdx.x & 31) == 0) s_min[threadIdx.x >> 5] = entry;
+  }
+  publish_block_count(kept, block_counts, group_counts);  // (its barrier orders the warp minima)
+  if (poses && threadIdx.x == 0) {
+    uint32_t m = s_min[0];
+    for (int w = 1; w < kThreads / 32; ++w) m = min(m, s_min[w]);
+    if (m != 0xffffffffu) atomicMin(pose_min, m);
+  }
 }
 
 // Ordered compaction (transform feedback semantics) of a surfel-indexed pass without a scan kernel: block b's offset =
@@ -1315,7 +1334,7 @@ void launch_compact_live(const Launch& L, SurfelPlanes src, const uint32_t* n_de
                          uint8_t* keep, uint32_t* block_counts, uint32_t* group_counts, SurfelPlanes dst, uint32_t* out) {
   if (n_upper > 0) {
     ScopedKernel sk(L, K_EXTRACT_FLAGS);
-    k_extract_flags<<<(n_upper + kThreads - 1) / kThreads, kThreads, 0, L.stream>>>(src, n_dev, live, nullptr,
+    k_extract_flags<<<(n_upper + kThreads - 1) / kThreads, kThreads, 0, L.stream>>>(src, n_dev, live, nullptr, 0u, nullptr,
                                                                                  make_float2(0.f, 0.f), 0.f, keep,
                                                                                  block_counts, group_counts);
   }
@@ -1328,13 +1347,15 @@ void launch_compact_live(const Launch& L, SurfelPlanes src, const uint32_t* n_de
 // downloads it to host RAM, SurfelMap.cpp:708-742). Slot s of the pool starts where slot s - 1 ends (slot 0 at 0);
 // rec[s] = {end of slot s in the pool, surfels of the tile}.
 void launch_extract_to_pool(const Launch& L, SurfelPlanes map, const uint32_t* n_dev, const uint8_t* live, uint32_t n_upper,
-                            const float* poses, float2 center, float extent, uint8_t* keep, uint32_t* block_counts,
+                            const float* poses, uint32_t pose_cap, uint32_t* pose_min, float2 center, float extent,
+                            uint8_t* keep, uint32_t* block_counts,
                             uint32_t* group_counts, SurfelPlanes pool, uint32_t pool_cap, uint2* rec, uint32_t slot,
                             uint32_t tile_cap) {
   if (n_upper > 0) {
     ScopedKernel sk(L, K_EXTRACT_FLAGS);
-    k_extract_flags<<<(n_upper + kThreads - 1) / kThreads, kThreads, 0, L.stream>>>(map, n_dev, live, poses, center, extent,
-                                                                                 keep, block_counts, group_counts);
+    k_extract_flags<<<(n_upper + kThreads - 1) / kThreads, kThreads, 0, L.stream>>>(map, n_dev, live, poses, pose_cap, pose_min,
+                                                                                 center, extent, keep, block_counts,
+                                                                                 group_counts);
   }
   launch_compact(L, map, keep, block_counts, group_counts, n_dev, n_upper, pool, nullptr, slot ? &rec[slot - 1].x : nullptr,
                  pool_cap, tile_cap, &rec[slot].x);
