@@ -1118,6 +1118,13 @@ int update_active_submaps(sb_ctx* c, const float* pose) {  // SurfelMap.cpp:744-
   return SB_OK;
 }
 
+// sb_map_update_debug's counts, as the reference's transform feedback counts them: the surfels the update emits and the
+// new ones gen_surfels emits (at most the room the updated ones leave), both before the submap window
+void set_update_counts(sb_ctx* c, const uint32_t* counts) {
+  c->n_updated = counts[9];
+  c->n_new = std::min(counts[10], kMaxSurfels - std::min(counts[9], kMaxSurfels));
+}
+
 // pose_dev / inv_dev != nullptr: pipeline mode -- the pose (and its pose-table entry) already lives on the device,
 // nothing is read back here; the caller finishes with map_update_finish() after its end-of-scan synchronisation.
 // index_fused: the post-ICP render of this scan has written the index keys unless the track-loss recovery ran (IndexFuse)
@@ -1157,6 +1164,7 @@ int map_update(sb_ctx* c, const float* pose, const sb_frame* frame, const Mat4* 
   const bool lazy = deferred && n > 0 && (uint64_t)c->n_holes * kDenseHoleFraction < n &&
                     (uint64_t)n + Pd <= kMaxSurfels;
   c->lazy_update = lazy;
+  SB_CUDA(c, cudaMemsetAsync(c->res->counts + 9, 0, 2 * sizeof(uint32_t), L.stream));
   // Dense: K6c + K6e predicate into T, then ordered compaction back into the map lanes: counts[1] = S', counts[2] = kept.
   // (A single-pass variant with decoupled look-back was measured twice and loses: round 1 with a 32-wide chain, round 2
   // with 256-wide windows that stop at the nearest inclusive prefix -- 80.2 us against 48.8 + 23.8 us for the two
@@ -1183,14 +1191,13 @@ int map_update(sb_ctx* c, const float* pose, const sb_frame* frame, const Mat4* 
     c->map_timestamp += 1;
     return SB_OK;
   }
-  uint32_t cnt[9];
-  if ((r = fetch_counts(c, cnt, 9))) return r;
+  uint32_t cnt[11];
+  if ((r = fetch_counts(c, cnt, 11))) return r;
   absorb_pose_min(c, cnt[8]);
   c->n_host = cnt[0];
   c->n_holes = 0;  // (dense)
   c->n_upper = cnt[0];
-  c->n_updated = cnt[2];
-  c->n_new = cnt[3];
+  set_update_counts(c, cnt);
   if ((r = update_active_submaps(c, pose))) return r;  // :547
   c->map_timestamp += 1;
   return SB_OK;
@@ -2151,8 +2158,7 @@ int sb_process_scan_timed(sb_ctx* c, const float* pts4, const float* labels, con
   c->n_host = rb.counts[0];
   c->n_holes = c->lazy_update ? rb.counts[5] : 0;
   c->n_upper = rb.counts[0];
-  c->n_updated = rb.counts[2];
-  c->n_new = rb.counts[3];
+  set_update_counts(c, rb.counts);
   absorb_pose_min(c, rb.counts[8]);
   if (rb.pose.gn_error) return gn_fail(c);
   if (!loop_ran) absorb_pose_block(c, rb, had_icp);  // (the loop-closure step has already done it, and chose currentPose_old_)

@@ -126,7 +126,9 @@ struct ResultBlock {
   char pad1[8192 - 4096 - 64 * sizeof(long long)];
   // [0] physical end of the surfel slots, [1] physical end after the update (base for new), [2] kept updated,
   // [3] kept new, [4] extracted, [5] dead slots below [1] after an in-place update, [6] / [7] end of the written range /
-  // number kept of a compaction of the map (not read back), [8] smallest pose-table entry the extraction passes saw
+  // number kept of a compaction of the map (not read back), [8] smallest pose-table entry the extraction passes saw,
+  // [9] / [10] surfels the update / the generation pass emit before the submap window (the reference's transform-feedback
+  // counts, sb_map_update_debug)
   uint32_t counts[16];
 };
 static_assert(offsetof(ResultBlock, sums) == 4096, "result block layout");

@@ -985,6 +985,7 @@ __global__ void __launch_bounds__(kThreads, 4) k_update_surfels(KParams kp, Surf
   const uint32_t n = *n_dev;
   if (kLazy && k == 0) counts[1] = n;
   bool kept = false;
+  bool valid_kept = false;  // valid at the end of the pass, before the submap window (the transform feedback's count)
   bool lv = false;
   // in place, the lanes are written by this kernel: plain loads, not the read-only path. The liveness byte is loaded
   // together with them (gating the lane loads on it would cost an L2 round trip per wave).
@@ -1124,6 +1125,7 @@ __global__ void __launch_bounds__(kThreads, 4) k_update_surfels(KParams kp, Surf
     }
     if (o1.w < kp.log_unstable && kp.use_stability) valid_out = false;
     if (valid_out && mark_integrated) integrated[dpix] = 1;
+    valid_kept = valid_out;
     kept = valid_out && submap_keep(ua.poses, kp.pose_cap, o0, o2, ua.submap_center, ua.submap_extent);
     const float4 o3 = avg_prob_set ? make_float4(p3.x, p3.y, p3.z, avg_prob) : p3;
     if (!kLazy) {
@@ -1143,6 +1145,9 @@ __global__ void __launch_bounds__(kThreads, 4) k_update_surfels(KParams kp, Surf
   if (!kLazy && k < n) keep[k] = kept ? 1 : 0;
   // (group totals are cleared by the per-pixel prologue of the map update)
   publish_block_count(kept, block_counts, group_counts);
+  // counts[9]: the surfels the update emits before the submap window (update_surfels.geom), cleared before the launch
+  const int n_valid = __syncthreads_count(valid_kept ? 1 : 0);
+  if (threadIdx.x == 0 && n_valid) atomicAdd(counts + 9, (uint32_t)n_valid);
 }
 
 // K6d + K6e in ONE pass: new surfels are appended in x-major pixel order behind the updated ones
@@ -1155,6 +1160,7 @@ __global__ void __launch_bounds__(kThreads) k_gen_compact(KParams kp, FrameDev f
   const uint32_t vb = block_ticket(lb);
   int t = (int)(vb * blockDim.x + threadIdx.x);
   bool kept = false;
+  bool generated = false;  // emitted by gen_surfels, before the submap window
   float4 o0, o1, o2, o3;
   o0 = o1 = o2 = o3 = make_float4(0.f, 0.f, 0.f, 0.f);
   if (t < kp.W * kp.H) {
@@ -1174,6 +1180,7 @@ __global__ void __launch_bounds__(kThreads) k_gen_compact(KParams kp, FrameDev f
     V3 v = mk3(V.x, V.y, V.z), n = mk3(N.x, N.y, N.z);
     V3 view_dir = divs3(neg3(v), len3(v));
     bool valid = !invalid && !integ && (dot3(n, view_dir) > 0.01f);
+    generated = valid;
     if (valid) {
       V3 ng = normalize3(n);
       float4 S = __ldg(f.semantic + pix);
@@ -1185,6 +1192,9 @@ __global__ void __launch_bounds__(kThreads) k_gen_compact(KParams kp, FrameDev f
       kept = submap_keep(poses, kp.pose_cap, o0, o2, center, extent);
     }
   }
+  // counts[10]: the new surfels before the submap window and the capacity, cleared before the update's launch
+  const int n_generated = __syncthreads_count(generated ? 1 : 0);
+  if (threadIdx.x == 0 && n_generated) atomicAdd(counts + 10, (uint32_t)n_generated);
   uint32_t block_count;
   const uint32_t rank = block_rank<kThreads>(kept, block_count);
   const uint32_t excl = lookback_exclusive(lb, vb, block_count);
