@@ -242,6 +242,44 @@ int sb_preprocess_deskew(sb_ctx* ctx, const float* pts4, const float* labels, co
  * SurfelMapping.cpp:325-331): start the host-to-device copy of the NEXT scan on a separate copy stream; a following
  * sb_process_scan with the same host pointers / count (on_device = 0) uses the staged copy. At most two scans staged. */
 int sb_prefetch_scan(sb_ctx* ctx, const float* pts4, const float* labels, const float* probs, uint32_t n);
+/* ---- per-point labels (no counterpart in the reference; DESIGN.md section 13) -------------------------------------
+ * With the mode on, every sb_process_scan / sb_process_scan_timed leaves one 32-byte record per input point, in input
+ * order, for SemanticKITTI-style tools that want one label per point. Every field is an exact function of the point and
+ * of what the scan computed:
+ *   pixel        y * data_width + x of the data pixel the projection gives the point (the deskewed point p' when
+ *                deskewing is on); -1 when the point enters no pixel: non-finite, the origin, clipped by the field of view
+ *                or the seam, z outside [-1, 1], or at the clear depth
+ *   flags        SB_POINT_WON: the pixel's depth test kept this point (ties: the lowest index, GL_LESS in buffer order);
+ *                SB_POINT_VERTEX: the frame's vertex at pixel has w > 0 (clear for the movable winner of a scan before
+ *                timestamp 10); SB_POINT_INTEGRATED: this scan's map update fused the pixel into an existing surfel (the
+ *                flag of sb_map_update_debug); SB_POINT_MAP: the model vertex at map_pixel has w > 0
+ *   frame_label / frame_prob  rintf(255 sem.x) and sem.w of the current frame's semantic image at pixel: the pixel's
+ *                label after the Q1 pairing, erosion and flood fill, not the point's own input label
+ *   map_pixel    y * model_width + x of p' under the model image's projection (no depth range); -1 when pixel is -1
+ *   map_label / map_prob / map_range  label and probability of the current model frame at map_pixel and |v| of its
+ *                vertex ((x*x + y*y) + z*z in fp32), when SB_POINT_MAP is set, else 0. That frame is the map after the
+ *                scan's update rendered at the scan's pose; with render_after_update = 0 there is none and the flag is
+ *                never set.
+ * Labels decode with one fp32 expression, so ids up to 65535 round-trip. */
+enum { SB_POINT_WON = 1, SB_POINT_VERTEX = 2, SB_POINT_INTEGRATED = 4, SB_POINT_MAP = 8 };
+typedef struct sb_point_label {
+  int32_t pixel;
+  uint32_t flags; /* SB_POINT_* */
+  uint32_t frame_label;
+  float frame_prob;
+  int32_t map_pixel;
+  uint32_t map_label;
+  float map_prob;
+  float map_range;
+} sb_point_label; /* 32 bytes */
+/* Valid at any time; kept across sb_reset; not part of a checkpoint (its bytes do not depend on the mode). With the mode
+ * off the scan pipeline launches exactly what it launches without this feature. Records exist from the first scan after
+ * the mode is turned on; sb_reset, sb_state_load, sb_set_params and turning the mode off drop them. The record buffer
+ * grows with the scan: a scan whose allocation fails returns SB_ERR_NOMEM before it changes anything. */
+int sb_set_point_labels(sb_ctx* ctx, int on);
+/* The records of the last scan. *n is always set (0 while none exist); SB_ERR_STATE while none exist, SB_ERR_INVALID
+ * (nothing written) when cap < *n. dst_on_device != 0: dst is device memory (a device-to-device copy). */
+int sb_get_point_labels(sb_ctx* ctx, sb_point_label* dst, uint32_t cap, uint32_t* n, int dst_on_device);
 /* ---- loop closure: SurfelMapping::checkLoopClosure, core/SurfelMapping.cpp:478-795 ("close-loops", default.xml:70-76) ----
  * When enabled, sb_process_scan runs the reference's detection / verification between updatePose() and updateMap()
  * (:196-200): render_inactive at a candidate pose, three Gauss-Newton runs against the old map frame, render_composed,

@@ -471,6 +471,16 @@ class SurfelMapping {
     check(sb_get_deskew(ctx_->get(), &d), ctx_->get(), "SurfelMapping::getDeskew");
     return d;
   }
+  /** per-point label records of every following scan (sb_set_point_labels; DESIGN.md section 13) */
+  void setPointLabels(bool on) { check(sb_set_point_labels(ctx_->get(), on ? 1 : 0), ctx_->get(), "SurfelMapping::setPointLabels"); }
+  /** the records of the last scan, one per input point in input order (sb_get_point_labels) */
+  void getPointLabels(std::vector<sb_point_label>& out) const {
+    uint32_t n = 0;
+    const int rc = sb_get_point_labels(ctx_->get(), nullptr, 0, &n, 0);
+    if (rc != SB_OK && !(rc == SB_ERR_INVALID && n > 0)) check(rc, ctx_->get(), "SurfelMapping::getPointLabels");
+    out.resize(n);
+    check(sb_get_point_labels(ctx_->get(), out.data(), n, &n, 0), ctx_->get(), "SurfelMapping::getPointLabels");
+  }
   void reset() {
     check(sb_reset(ctx_->get()), ctx_->get(), "SurfelMapping::reset");
     trajectory_.clear();

@@ -13,6 +13,7 @@ import numpy as np
 from . import build as _build
 
 SB_OK = 0
+SB_ERR_INVALID = -1
 _ERRORS = {-1: "SB_ERR_INVALID", -2: "SB_ERR_CUDA", -3: "SB_ERR_NOMEM", -4: "SB_ERR_CAPACITY", -5: "SB_ERR_STATE",
            -6: "SB_ERR_NOGPU"}
 
@@ -62,6 +63,19 @@ def deskew_params(mode="off", ref_time=0.5, start_azimuth=np.pi, clockwise=True)
     d.mode = DESKEW_MODES.get(mode, mode) if isinstance(mode, str) else int(mode)
     d.ref_time, d.start_azimuth, d.clockwise = ref_time, start_azimuth, 1 if clockwise else 0
     return d
+
+
+class PointLabel(C.Structure):  # sb_point_label
+    _fields_ = [("pixel", C.c_int32), ("flags", C.c_uint32), ("frame_label", C.c_uint32), ("frame_prob", C.c_float),
+                ("map_pixel", C.c_int32), ("map_label", C.c_uint32), ("map_prob", C.c_float), ("map_range", C.c_float)]
+
+
+# sb_point_label as a numpy structured dtype (same names, offsets and 32-byte size) and its flags
+POINT_LABEL_DTYPE = np.dtype({"names": [n for n, _ in PointLabel._fields_],
+                              "formats": ["<i4", "<u4", "<u4", "<f4", "<i4", "<u4", "<f4", "<f4"],
+                              "offsets": [getattr(PointLabel, n).offset for n, _ in PointLabel._fields_],
+                              "itemsize": C.sizeof(PointLabel)})
+POINT_WON, POINT_VERTEX, POINT_INTEGRATED, POINT_MAP = 1, 2, 4, 8
 
 
 class Params(C.Structure):
@@ -177,6 +191,7 @@ def lib(build_if_missing=True):
         "sb_set_deskew": [vp, C.POINTER(DeskewParams)], "sb_get_deskew": [vp, C.POINTER(DeskewParams)],
         "sb_process_scan_timed": [vp, vp, vp, vp, vp, u32, C.c_int],
         "sb_preprocess_deskew": [vp, vp, vp, vp, vp, u32, u32, C.POINTER(DeskewParams), pd, C.c_int, vp],
+        "sb_set_point_labels": [vp, C.c_int], "sb_get_point_labels": [vp, vp, u32, C.POINTER(u32), C.c_int],
     }
     for name, args in sig.items():
         fn = getattr(L, name)
@@ -210,6 +225,7 @@ EXPORTED_SYMBOLS = [
     "sb_profile_kernels", "sb_profile_name", "sb_profile_collect", "sb_state_size", "sb_state_save", "sb_state_load",
     "sb_set_tile_cache", "sb_get_tile_cache_info",
     "sb_default_deskew", "sb_set_deskew", "sb_get_deskew", "sb_process_scan_timed", "sb_preprocess_deskew",
+    "sb_set_point_labels", "sb_get_point_labels",
 ]
 
 
@@ -709,6 +725,27 @@ class SurfelMapping:
         rc = lib().sb_prefetch_scan(self.ctx.h, C.c_void_p(ptr_pts), C.c_void_p(ptr_labels) if ptr_labels else None,
                                     C.c_void_p(ptr_probs) if ptr_probs else None, n)
         self.ctx.check(rc, "prefetch_scan")
+
+    def setPointLabels(self, on=True):
+        """Per-point label records of every following scan (sb_set_point_labels; DESIGN.md section 13)"""
+        self.ctx.check(lib().sb_set_point_labels(self.ctx.h, 1 if on else 0), "set_point_labels")
+
+    def getPointLabels(self, out=None):
+        """The records of the last scan, one per input point in input order: a numpy structured array of
+        POINT_LABEL_DTYPE (the fields of sb_point_label). out: an int device pointer to n * 32 bytes to fill instead
+        (device-to-device copy); then returns n."""
+        n = C.c_uint32(0)
+        rc = lib().sb_get_point_labels(self.ctx.h, None, 0, C.byref(n), 0)
+        if rc != SB_OK and not (rc == SB_ERR_INVALID and n.value > 0):
+            self.ctx.check(rc, "get_point_labels")
+        if out is not None:
+            self.ctx.check(lib().sb_get_point_labels(self.ctx.h, C.c_void_p(out), n.value, C.byref(n), 1),
+                           "get_point_labels")
+            return int(n.value)
+        a = np.zeros(n.value, POINT_LABEL_DTYPE)
+        self.ctx.check(lib().sb_get_point_labels(self.ctx.h, _vp(a) if a.size else None, n.value, C.byref(n), 0),
+                       "get_point_labels")
+        return a
 
     def getCurrentPose(self):
         a = np.zeros(16)

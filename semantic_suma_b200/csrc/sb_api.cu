@@ -20,6 +20,8 @@
 
 using namespace sb;
 
+static_assert(sizeof(sb_point_label) == 32 && offsetof(sb_point_label, map_pixel) == 16, "sb_point_label layout");
+
 struct sb_frame {
   sb_ctx* ctx;
   uint64_t id;  // unique within the context, never reused (keys the render memo)
@@ -126,6 +128,13 @@ struct sb_ctx {
   DevPtr<float4> d_desk;
   DevPtr<float> d_times;
   size_t desk_cap = 0;
+  // per-point labels (sb_set_point_labels; DESIGN.md section 13): off by default, kept across sb_reset, never saved. The
+  // records of the last scan (pl_valid) live in a buffer of pl_cap records, allocated on the first scan that needs it.
+  bool point_labels = false;
+  bool pl_valid = false;
+  uint32_t pl_n = 0;
+  DevPtr<sb_point_label> pl_buf;
+  size_t pl_cap = 0;
 
   // ---- ICP
   DevPtr<GnState> gn;
@@ -456,6 +465,7 @@ int reset_state(sb_ctx* c) {
   memset(c->stats, 0, sizeof(c->stats));
   c->trackLoss = 0;
   c->n_upper = 0;
+  c->pl_valid = false;
   {
     // staged in the context's own pinned buffer (read by the async copy until the synchronize at the end of this
     // function; no other transfer of this context is in flight here): contexts reset concurrently share nothing
@@ -1327,6 +1337,31 @@ int setup_deskew(sb_ctx* c, const sb_deskew_params& d, const double* M, const fl
   return SB_OK;
 }
 
+// ---- per-point labels (DESIGN.md section 13) ----
+// the record buffer grows like the point buffers; the old buffer may still be written by the scan in flight
+int reserve_point_labels(sb_ctx* c, size_t n) {
+  if (n <= c->pl_cap) return SB_OK;
+  const size_t cap = std::max(c->pts_cap, n + n / 4 + 1024);
+  SB_CUDA(c, cudaStreamSynchronize(c->stream));
+  DevPtr<sb_point_label> nb;
+  if (dev_alloc(nb, cap * sizeof(sb_point_label)) != cudaSuccess) {
+    cudaGetLastError();
+    return fail(c, SB_ERR_NOMEM, "out of device memory for the per-point label records");
+  }
+  c->pl_buf = std::move(nb);
+  c->pl_cap = cap;
+  return SB_OK;
+}
+
+// the records of the scan in c->cur from its points, key image (the one launch_preprocess read last), frame, integrated
+// flags and, when this scan rendered one, its model frame
+void enqueue_point_labels(sb_ctx* c, const float4* pts, uint32_t n, const DeskewArgs* deskew) {
+  const PrepKeys& k = c->prep;
+  PointLabelIO io{pts, n, k.img[k.cur ^ 1], c->cur->d, c->integrated,
+                  c->p.render_after_update ? c->cur_model->d : null_frame(), c->pl_buf};
+  launch_point_labels(L_(c), c->kp, io, deskew);
+}
+
 // SurfelMap::render_composed, SurfelMap.cpp:1116-1165
 int render_composed_internal(sb_ctx* c, const float* pose_old, const float* pose_new, float conf_thr) {
   frame_written(c, c->f_comp);
@@ -1701,6 +1736,7 @@ int sb_set_params(sb_ctx* c, const sb_params* p) {
   c->p = *p;
   derive(c);
   c->memo.clear();
+  c->pl_valid = false;
   return SB_OK;
 }
 
@@ -2105,6 +2141,8 @@ int sb_process_scan_timed(sb_ctx* c, const float* pts4, const float* labels, con
   int r = upload_scan(c, pts4, labels, probs, n, on_device, &dp, &dl, &dq);
   if (r) return r;
   if ((r = reserve_poses(c, (uint64_t)c->map_timestamp + 1))) return r;  // the entry this scan writes
+  if (c->point_labels && (r = reserve_point_labels(c, n))) return r;
+  c->pl_valid = false;
   // deskewing with the motion the next Gauss-Newton run starts from: lastIncrement_ as the previous scan left it
   DeskewArgs da;
   bool deskew = false;
@@ -2146,6 +2184,7 @@ int sb_process_scan_timed(sb_ctx* c, const float* pts4, const float* labels, con
   if (p.render_after_update) {
     if ((r = render_full(c, nullptr, nullptr, ct2, c->cur_model, &c->res->pose.invP_cur, true))) return r;
   }
+  if (c->point_labels) enqueue_point_labels(c, dp, n, deskew ? &da : nullptr);
   // ---- the scan's results: pose block, statistics sums, surfel counts ----
   const ResultBlock& rb = c->host->result;
   SB_CUDA(c, cudaMemcpyAsync(&c->host->result, c->res, sizeof(ResultBlock), cudaMemcpyDeviceToHost, c->stream));
@@ -2173,8 +2212,18 @@ int sb_process_scan_timed(sb_ctx* c, const float* pts4, const float* labels, con
   {
     const uint32_t n0 = c->n_host;
     if ((r = update_active_submaps(c, P_cur.m))) return r;
-    if (c->n_host != n0 && p.render_after_update && (r = render_full(c, P_cur.m, P_cur.m, ct2, c->cur_model))) return r;
+    if (c->n_host != n0 && p.render_after_update) {
+      if ((r = render_full(c, P_cur.m, P_cur.m, ct2, c->cur_model))) return r;
+      // the records read the model frame: label the scan again from the new one, finished before the call returns
+      // (the caller's device points may change after it)
+      if (c->point_labels) {
+        enqueue_point_labels(c, dp, n, deskew ? &da : nullptr);
+        SB_CUDA(c, cudaStreamSynchronize(c->stream));
+      }
+    }
   }
+  c->pl_n = n;
+  c->pl_valid = c->point_labels;
   c->stats[7] = n_live(c);
   // The reference's three stage timers (preprocessing / icp / mapping) have no meaning here -- the stages overlap on
   // the stream; the slots carry the host-side split of the call instead: enqueue, wait for the device, bookkeeping.
@@ -2184,6 +2233,27 @@ int sb_process_scan_timed(sb_ctx* c, const float* pts4, const float* labels, con
   c->stats[10] = t_end - t_synced;
   c->stats[11] = t_end - t_all;
   c->timestamp += 1;
+  return SB_OK;
+}
+
+int sb_set_point_labels(sb_ctx* c, int on) {
+  if (!c) return SB_ERR_INVALID;
+  c->point_labels = on != 0;
+  if (!c->point_labels) c->pl_valid = false;
+  return SB_OK;
+}
+
+int sb_get_point_labels(sb_ctx* c, sb_point_label* dst, uint32_t cap, uint32_t* n, int dst_on_device) {
+  if (!c || !n) return SB_ERR_INVALID;
+  *n = c->pl_valid ? c->pl_n : 0;
+  if (!c->pl_valid) return fail(c, SB_ERR_STATE, "get_point_labels: no records (mode off, or no scan since it was turned "
+                                                 "on or since the last reset, load or set_params)");
+  if (cap < c->pl_n || (!dst && c->pl_n)) return fail(c, SB_ERR_INVALID, "get_point_labels: buffer smaller than the scan");
+  cudaSetDevice(c->device);
+  if (c->pl_n)
+    SB_CUDA(c, cudaMemcpyAsync(dst, c->pl_buf, (size_t)c->pl_n * sizeof(sb_point_label),
+                               dst_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, c->stream));
+  SB_CUDA(c, cudaStreamSynchronize(c->stream));
   return SB_OK;
 }
 
@@ -3276,6 +3346,7 @@ int sb_state_load(sb_ctx* c, const void* src, uint64_t n) {
   // the pose tables take the checkpoint's size (no change when the allocation fails)
   if (s.pose_cap != c->pose_cap && (r = resize_pose_tables(c, s.pose_cap, 0))) return r;
   // ---- the header is sound: from here on the context changes ----
+  c->pl_valid = false;
   if ((r = discard_prefetch(c))) return r;
   if ((r = state_staging(c))) return r;
   const uint8_t* in = static_cast<const uint8_t*>(src);

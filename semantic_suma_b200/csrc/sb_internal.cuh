@@ -164,7 +164,7 @@ enum KernelId {
   K_FILL = 0, K_PROJECT_SCATTER, K_PREPROCESS_TILE, K_ICP_JACOBIAN, K_GN_INIT,
   K_ICP_FUSED, K_POSE_PRODUCTS, K_RENDER_SCATTER, K_RENDER_RESOLVE, K_INDEX_SCATTER, K_RADIUS, K_UPDATE_SURFELS,
   K_GEN_SURFELS, K_EXTRACT_FLAGS, K_COMPACT_SCATTER, K_AOS_TO_SOA, K_SOA_TO_AOS, K_ICP_POST, K_STATE_PACK,
-  K_STATE_UNPACK, K_STATE_DIGEST, K_POOL_RECLAIM, K_COUNT
+  K_STATE_UNPACK, K_STATE_DIGEST, K_POOL_RECLAIM, K_POINT_LABELS, K_COUNT
 };
 const char* kernel_name(int id);
 
@@ -230,6 +230,18 @@ void launch_preprocess(const Launch& L, const KParams& kp, const float4* pts, co
                        uint32_t n, uint32_t timestamp, PrepKeys& keys, FrameDev out, float4* radius_map,
                        unsigned long long* index_keys, uint8_t* integrated, uint32_t* group_counts,
                        const DeskewArgs* deskew = nullptr);
+// per-point labels of a scan (DESIGN.md section 13): the scan's own points, its key image (the one launch_preprocess
+// read), its data frame and integrated flags, and the model frame (model.vertex == nullptr: none this scan)
+struct PointLabelIO {
+  const float4* pts;
+  uint32_t n;
+  const unsigned long long* keys;
+  FrameDev frame;
+  const uint8_t* integrated;
+  FrameDev model;
+  sb_point_label* out;
+};
+void launch_point_labels(const Launch& L, const KParams& kp, const PointLabelIO& io, const DeskewArgs* deskew);
 
 // sb_icp.cu
 void launch_icp_jacobian(const Launch& L, const KParams& kp, const IcpArgs& a, const Mat4& pose, int iteration,

@@ -27,7 +27,8 @@ const char* kernel_name(int id) {
                                        "icp_jacobian", "gn_init", "icp_fused", "pose_products", "render_scatter",
                                        "render_resolve", "index_scatter", "radius", "update_surfels", "gen_surfels",
                                        "extract_flags", "compact_scatter", "aos_to_soa", "soa_to_aos", "icp_post",
-                                       "state_pack", "state_unpack", "state_digest", "pool_reclaim"};
+                                       "state_pack", "state_unpack", "state_digest", "pool_reclaim",
+                                       "point_labels"};
   return (id >= 0 && id < K_COUNT) ? names[id] : "?";
 }
 

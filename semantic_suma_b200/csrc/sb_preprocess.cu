@@ -12,14 +12,10 @@
 namespace sb {
 using namespace sbm;
 
-// K1a: gen_vertexmap.vert:73-91 -- one thread per point, scatter-min into the key image.
-// kDeskew: the point is first moved to the scan's reference time (DESIGN.md section 11) and written to dk.out, from where
-// k_preprocess_tile reads the winners; the off instance does not touch dk.
+// ---- K1a's per-point body, shared by the scatter and by the per-point labels (one source for the pixel arithmetic) ----
+// The point i as the projection sees it. kDeskew: moved to the scan's reference time (DESIGN.md section 11).
 template <bool kDeskew>
-__global__ void __launch_bounds__(256) k_project_scatter(KParams kp, const float4* __restrict__ pts, uint32_t n,
-                                                         unsigned long long* __restrict__ keys, DeskewArgs dk) {
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
+__device__ __forceinline__ float4 k1_point(const float4* __restrict__ pts, uint32_t i, const DeskewArgs& dk) {
   float4 p4 = __ldg(pts + i);
   if (kDeskew) {
     const float s = deskew_sweep_time(dk.mode, dk.mode == 1 ? __ldg(dk.times + i) : 0.0f,
@@ -28,24 +24,51 @@ __global__ void __launch_bounds__(256) k_project_scatter(KParams kp, const float
     const V3 q = deskew_point(mk3(p4.x, p4.y, p4.z), s - dk.ref_time, mk3(dk.w[0], dk.w[1], dk.w[2]),
                               mk3(dk.t[0], dk.t[1], dk.t[2]));
     p4 = make_float4(q.x, q.y, q.z, p4.w);
-    dk.out[i] = p4;
   }
-  V3 pos = mk3(p4.x, p4.y, p4.z);
-  float d = len3(pos);
+  return p4;
+}
+
+// gen_vertexmap.vert:83-89: the pixel (ix, iy) of pos at range d in a W x H image under (fov_up, fov); false: clipped
+// (field of view, the seam at yaw -pi, NaN)
+__device__ __forceinline__ bool k1_pixel(V3 pos, float d, int W, int H, float fov_up, float fov, int* ix, int* iy) {
   float yaw = atan2f_(pos.y, pos.x);
   float pitch = -asinf_(pos.z / d);
   float x = -yaw * kInvPi;
-  float y = 1.0f - (2.0f * (kRad2Deg * pitch + kp.fov_up)) / kp.fov;
-  float z = 2.0f * ((d - kp.min_depth) / (kp.max_depth - kp.min_depth)) - 1.0f;
-  float fx = floorf((0.5f * (x + 1.0f)) * (float)kp.W);
-  float fy = floorf((0.5f * (y + 1.0f)) * (float)kp.H);
-  if (!(fx >= 0.0f && fx < (float)kp.W && fy >= 0.0f && fy < (float)kp.H)) return;  // clipped
-  if (!(z >= -1.0f && z <= 1.0f)) return;
-  uint32_t d24 = depth24(0.5f * z + 0.5f);
-  if (d24 >= kDepthClear) return;  // GL_LESS against the cleared buffer
+  float y = 1.0f - (2.0f * (kRad2Deg * pitch + fov_up)) / fov;
+  float fx = floorf((0.5f * (x + 1.0f)) * (float)W);
+  float fy = floorf((0.5f * (y + 1.0f)) * (float)H);
+  if (!(fx >= 0.0f && fx < (float)W && fy >= 0.0f && fy < (float)H)) return false;
+  *ix = (int)fx;
+  *iy = (int)fy;
+  return true;
+}
+
+// gen_vertexmap.vert:85-91: the data pixel and 24-bit depth of pos; false when the point scatters no key
+__device__ __forceinline__ bool k1_project(const KParams& kp, V3 pos, int* ix, int* iy, uint32_t* d24) {
+  const float d = len3(pos);
+  if (!k1_pixel(pos, d, kp.W, kp.H, kp.fov_up, kp.fov, ix, iy)) return false;
+  const float z = 2.0f * ((d - kp.min_depth) / (kp.max_depth - kp.min_depth)) - 1.0f;
+  if (!(z >= -1.0f && z <= 1.0f)) return false;
+  *d24 = depth24(0.5f * z + 0.5f);
+  return *d24 < kDepthClear;  // GL_LESS against the cleared buffer
+}
+
+// K1a: gen_vertexmap.vert:73-91 -- one thread per point, scatter-min into the key image.
+// kDeskew: the moved point is also written to dk.out, from where k_preprocess_tile reads the winners; the off instance
+// does not touch dk.
+template <bool kDeskew>
+__global__ void __launch_bounds__(256) k_project_scatter(KParams kp, const float4* __restrict__ pts, uint32_t n,
+                                                         unsigned long long* __restrict__ keys, DeskewArgs dk) {
+  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float4 p4 = k1_point<kDeskew>(pts, i, dk);
+  if (kDeskew) dk.out[i] = p4;
+  int ix, iy;
+  uint32_t d24;
+  if (!k1_project(kp, mk3(p4.x, p4.y, p4.z), &ix, &iy, &d24)) return;
   // key image rows are [W + 6]: three mirror columns on both sides (see k_preprocess_tile)
-  const int ix = (int)fx, Wp = kp.W + 6;
-  unsigned long long* row = keys + (size_t)(int)fy * Wp;
+  const int Wp = kp.W + 6;
+  unsigned long long* row = keys + (size_t)iy * Wp;
   const unsigned long long key = ((unsigned long long)d24 << 32) | (unsigned long long)i;
   atomicMin(row + ix + 3, key);
   if (ix < 3) atomicMin(row + ix + 3 + kp.W, key);
@@ -313,6 +336,66 @@ void launch_preprocess(const Launch& L, const KParams& kp, const float4* pts, co
       k_preprocess_tile<false><<<grid, kPrepThreads, 0, L.stream>>>(kp, io, keys.tmap[keys.cur]);
   }
   keys.cur ^= 1;
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// Per-point labels (DESIGN.md section 13): one thread per point, after the scan's last model render. The key image the
+// scan's tile pass read stays untouched until the next scan's tile pass re-arms it (nothing else writes PrepKeys), so
+// WON is the comparison of the point's own key with the pixel's.
+// ------------------------------------------------------------------------------------------------------------
+// rintf(255 x) as an unsigned id; NaN and negatives give 0, values past the range saturate (the oracle's rule)
+__device__ __forceinline__ uint32_t label_id(float x) {
+  const float f = rintf(x * 255.0f);
+  return f > 0.0f ? (f < 4294967296.0f ? (uint32_t)f : 0xffffffffu) : 0u;
+}
+
+template <bool kDeskew>
+__global__ void __launch_bounds__(256) k_point_labels(KParams kp, PointLabelIO io, DeskewArgs dk) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= io.n) return;
+  const float4 p4 = k1_point<kDeskew>(io.pts, i, dk);
+  const V3 pos = mk3(p4.x, p4.y, p4.z);
+  int pixel = -1, map_pixel = -1;
+  uint32_t flags = 0, frame_label = 0, map_label = 0;
+  float frame_prob = 0.0f, map_prob = 0.0f, map_range = 0.0f;
+  int ix, iy;
+  uint32_t d24;
+  if (k1_project(kp, pos, &ix, &iy, &d24)) {
+    pixel = iy * kp.W + ix;
+    const unsigned long long key = ((unsigned long long)d24 << 32) | (unsigned long long)i;
+    if (io.keys[(size_t)iy * (kp.W + 6) + ix + 3] == key) flags |= SB_POINT_WON;
+    if (io.frame.vertex[pixel].w > 0.0f) flags |= SB_POINT_VERTEX;
+    if (io.integrated[pixel]) flags |= SB_POINT_INTEGRATED;
+    const float4 s = io.frame.semantic[pixel];
+    frame_label = label_id(s.x);
+    frame_prob = s.w;
+    int mx, my;
+    if (k1_pixel(pos, len3(pos), kp.Wm, kp.Hm, kp.m_fov_up, kp.m_fov, &mx, &my)) {
+      map_pixel = my * kp.Wm + mx;
+      if (io.model.vertex) {
+        const float4 mv = io.model.vertex[map_pixel];
+        if (mv.w > 0.0f) {
+          const float4 ms = io.model.semantic[map_pixel];
+          flags |= SB_POINT_MAP;
+          map_label = label_id(ms.x);
+          map_prob = ms.w;
+          map_range = len3(mk3(mv.x, mv.y, mv.z));
+        }
+      }
+    }
+  }
+  uint4* out = reinterpret_cast<uint4*>(io.out + i);  // 32 bytes: two 16-byte stores
+  out[0] = make_uint4((uint32_t)pixel, flags, frame_label, __float_as_uint(frame_prob));
+  out[1] = make_uint4((uint32_t)map_pixel, map_label, __float_as_uint(map_prob), __float_as_uint(map_range));
+}
+
+void launch_point_labels(const Launch& L, const KParams& kp, const PointLabelIO& io, const DeskewArgs* deskew) {
+  if (io.n == 0) return;
+  ScopedKernel sk(L, K_POINT_LABELS);
+  if (deskew)
+    k_point_labels<true><<<(io.n + 255) / 256, 256, 0, L.stream>>>(kp, io, *deskew);
+  else
+    k_point_labels<false><<<(io.n + 255) / 256, 256, 0, L.stream>>>(kp, io, DeskewArgs{});
 }
 
 }  // namespace sb

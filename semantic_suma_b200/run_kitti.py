@@ -18,6 +18,11 @@ Full sequences extract more submap tiles than the default HBM tile cache holds: 
 cache (sb_set_tile_cache) with up to N surfels in pinned host memory (inf: no bound, as the reference's cache; 0: the
 default cache). The run then prints the cache's counters.
 
+--write-labels DIR (with --semantic) writes DIR/NNNNNN.label per scan in the SemanticKITTI format: one uint32 per input
+point, the label the fused map gives the point in the low 16 bits (0, unlabeled, where the map has no surfel at the
+point's pixel) and instance 0 (sb_get_point_labels; DESIGN.md section 13). A resumed run writes the files from the scan
+after the checkpoint on, byte-identical to those of an uninterrupted run.
+
 The engine is the CUDA library (an H100 is required); tests inject another engine through `make_engine` to check the
 file plumbing without a GPU.
 """
@@ -80,10 +85,16 @@ def parse_host_surfels(text):
 
 
 TILE_POOL_SURFELS = 16 * 1024 * 1024  # the HBM share of a managed tile cache: the whole pool
+POINT_MAP = 8  # sb_point_label flag: the model frame has a surfel at the point's pixel
+
+
+def map_label_ids(records):
+    """the SemanticKITTI id of every point of a scan: the map's label where it has one, 0 (unlabeled) elsewhere"""
+    return np.where(records["flags"] & POINT_MAP, records["map_label"], 0).astype(np.uint32)
 
 
 def run_sequence(seq_dir, params, make_engine=None, semantic=False, max_scans=None, on_scan=None, save_state=None,
-                 save_every=None, resume=None, tile_cache_host=0, deskew="off"):
+                 save_every=None, resume=None, tile_cache_host=0, deskew="off", write_labels=None):
     """-> dict(poses=[4x4 float64 in the velodyne frame, from scan 0], seconds, scans processed by this call, and
     tile_cache: the cache's counters when tile_cache_host is set).
     `make_engine(params)` must return an object with processScan(points4, labels, probs) and getCurrentPose() -- the
@@ -92,7 +103,9 @@ def run_sequence(seq_dir, params, make_engine=None, semantic=False, max_scans=No
     resume: a checkpoint written by save_state; the run continues at the scan after it (with the cache it was saved with).
     tile_cache_host: surfels the managed tile cache may keep in host memory (inf: no bound; 0: the default cache).
     deskew: "off" or "azimuth" (per-point deskewing by each point's azimuth, setDeskew); a resumed run keeps the setting
-    of its checkpoint."""
+    of its checkpoint.
+    write_labels: a directory for one SemanticKITTI .label file per scan from the map's labels (map_label_ids); the
+    engine then needs setPointLabels(on) and getPointLabels() (records with the fields of sb_point_label)."""
     files = list_scans(seq_dir)
     if max_scans is not None:
         files = files[:max_scans]
@@ -103,6 +116,9 @@ def run_sequence(seq_dir, params, make_engine=None, semantic=False, max_scans=No
         engine.setTileCache(TILE_POOL_SURFELS, tile_cache_host)
     if deskew != "off":
         engine.setDeskew(deskew)
+    if write_labels:
+        os.makedirs(write_labels, exist_ok=True)
+        engine.setPointLabels(True)
     poses = read_checkpoint(engine, resume) if resume else []
     first = len(poses)
     if first > len(files):
@@ -117,6 +133,9 @@ def run_sequence(seq_dir, params, make_engine=None, semantic=False, max_scans=No
             lf = os.path.join(seq_dir, "labels", os.path.splitext(os.path.basename(f))[0] + ".label")
             labels, probs = kitti.read_labels(lf, n_points=pts.shape[0])
         engine.processScan(pts, labels, probs)
+        if write_labels:
+            name = os.path.splitext(os.path.basename(f))[0] + ".label"
+            kitti.write_labels(os.path.join(write_labels, name), map_label_ids(engine.getPointLabels()))
         poses.append(np.asarray(engine.getCurrentPose(), np.float64).copy())
         if on_scan:
             on_scan(i, poses[-1])
@@ -190,9 +209,13 @@ def main(argv=None, make_engine=None):
     ap.add_argument("--deskew", choices=("off", "azimuth"), default="off",
                     help="per-point deskewing by azimuth (off for KITTI odometry, whose scans are treated as already "
                          "motion-compensated)")
+    ap.add_argument("--write-labels", default=None, metavar="DIR",
+                    help="write DIR/NNNNNN.label per scan: the fused map's label of every point (needs --semantic)")
     args = ap.parse_args(argv)
     if args.save_every is not None and (args.save_every <= 0 or not args.save_state):
         ap.error("--save-every needs --save-state and N > 0")
+    if args.write_labels and not args.semantic:
+        ap.error("--write-labels needs --semantic")
     if args.make_synthetic:
         make_synthetic_sequence(args.make_synthetic, args.scans, width=args.width, semantic=args.semantic)
         print("wrote", args.make_synthetic)
@@ -204,7 +227,7 @@ def main(argv=None, make_engine=None):
     params = api.default_params(data_width=args.width, model_width=args.width)
     res = run_sequence(args.seq, params, make_engine=make_engine, semantic=args.semantic, max_scans=args.max_scans,
                        save_state=args.save_state, save_every=args.save_every, resume=args.resume,
-                       tile_cache_host=args.tile_cache_host, deskew=args.deskew)
+                       tile_cache_host=args.tile_cache_host, deskew=args.deskew, write_labels=args.write_labels)
     calib_file = os.path.join(args.seq, "calib.txt")
     Tr = kitti.read_calibration(calib_file).get("Tr") if os.path.exists(calib_file) else None
     if args.out:

@@ -93,7 +93,7 @@ class Scene:
         self.daz = 2.0 * np.pi / width
         self.delv = np.deg2rad(fov) / height
 
-    def scan(self, frame, pose=None, rolling=None, ref_time=0.5):
+    def scan(self, frame, pose=None, rolling=None, ref_time=0.5, clean_labels=False):
         """Returns (pts[N,4] float32 (x,y,z,1) in the sensor frame, labels[N] float32, probs[N] float32).
         Point order: azimuth-major, beams inner (as io/SimulationReader.cpp:103-116 builds its beam table).
 
@@ -101,7 +101,10 @@ class Scene:
         is measured at sweep time s_k = (k + 0.5) / W (column 0 first, as a clockwise spin starting at yaw +pi) from
         pose . D(s_k), D(s) = (Exp((s - ref_time) w), (s - ref_time) t) with (w, t) = (log R, t) of the increment; the
         points come back in that instantaneous sensor frame and a fourth array holds their s_k. The same seed gives the
-        same noise and, with rolling=None, exactly the output of a plain scan."""
+        same noise and, with rolling=None, exactly the output of a plain scan.
+
+        clean_labels (semantic scenes): one more array at the end, the labels before the 2 % random flips; every other
+        output is unchanged."""
         rng = np.random.default_rng(self.seed + frame)
         if pose is None:
             pose = trajectory(frame + 1)[-1]
@@ -158,10 +161,11 @@ class Scene:
         labels = np.where(hk == 0, 40.0, 50.0).astype(np.float32)
         for b in _CAR_BOXES:
             labels[hk == 1 + b] = 10.0
+        clean = labels.copy()
         flips = rng.random(labels.shape[0]) < 0.02
         labels[flips] = rng.choice(np.array([10.0, 40.0, 50.0, 70.0, 30.0], np.float32), int(flips.sum()))
         probs = rng.uniform(0.6, 1.0, labels.shape[0]).astype(np.float32)
-        return (pts, labels, probs) + extra
+        return (pts, labels, probs) + extra + ((clean,) if clean_labels else ())
 
 
 def make_sequence(n_frames, **kw):
